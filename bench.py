@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py — images/sec of the txt2img hot path (CFG denoising loop + VAE decode), the metric BASELINE.json names.
 
-  python bench.py --gpus N --steps K --warmup W [--config sd15|sdxl] [--dtype bf16|fp16] [--impl sdxe|reference] [--only-headline]
+  python bench.py --gpus N --steps K --warmup W [--config sd15|sdxl|c4] [--dtype bf16|fp16] [--impl sdxe|reference]
+                  [--only-headline] [--cpu-baseline] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch: `process_images` of B images. ONE invocation measures the whole
 metric and prints ONE JSON line:
@@ -13,14 +14,21 @@ metric and prints ONE JSON line:
     bit for bit (N = 1: a repeated run of its own batch).
 Weights are random-init of the exact architecture, conditioning is synthetic. N>1: one process per GPU (torchrun),
 images sharded one block per rank, ONE NCCL broadcast of each packed weight blob at load, no per-step collective (weak
-scaling). The sub-blocks time min(K, 5) steps after 2 warm-ups so that the default run stays within minutes.
+scaling). The headline times exactly K steps; the sub-blocks time min(K, 5) (c4: min(K, 3)) after 3 warm-ups so that a
+run stays within a few minutes, and each block reports its own `steps`.
 
 Every block carries `value` (inputs resident in HBM, result left on the device) and `e2e` (same call with pinned HOST
 conditioning copied in and uint8 images copied out inside the timed region); the headline and "sdxl" also carry
-`roofline` of the dominant kernel class (tcgen05 GEMM / implicit-GEMM conv; per-launch CUDA-event timing from one extra
+`roofline` of the dominant kernel class (wgmma GEMM / implicit-GEMM conv; per-launch CUDA-event timing from one extra
 instrumented pass after the timed region), `torch_sdp_gpu` (the reference's default-SDP GPU path restated in PyTorch,
-same box, same run) and `cpu_baseline` (oracle = the reference's `--use-cpu all --no-half` arithmetic on the host
-cores, bounded sample). `--impl reference` times only the CPU reference arm.
+same GPU, same run) and, with --cpu-baseline, `cpu_baseline` (oracle = the reference's `--use-cpu all --no-half`
+arithmetic on the host cores, bounded sample). That leg spends ~100 s of host time on full-size CPU UNet calls (8-core
+host: a whole run 291 s with it, 187 s without, at --steps 3), so it is opt-in; `--impl reference` times only the CPU
+reference arm.
+
+--dump-outputs DIR writes, after the timed steps, what the headline's last timed step returned (final latents and the
+uint8 images, as float32 .npy). With --gpus N > 1 only rank 0 writes, so DIR holds rank 0's shard (images 0 .. B-1). Inputs (weights, conditioning, seeds) are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -56,18 +64,23 @@ WORKLOADS = {
 }
 
 
+# NVIDIA H100 SXM data sheet, dense BF16 and HBM3 bandwidth at 700 W: a ceiling, not a rate any run has reached
+H100_PEAKS = dict(tflops=989.0, hbm_gbs=3350.0)
+
+
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return dict(tflops_sustained=d.get("bf16_tflops_sustained", 1400.0), tflops_burst=d.get("bf16_tflops", 1590.0),
-                    hbm_gbs=d.get("hbm_gbs", 6650.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(tflops_sustained=1400.0, tflops_burst=1590.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+        return dict(tflops_sustained=d.get("bf16_tflops_sustained", H100_PEAKS["tflops"]), tflops_burst=d.get("bf16_tflops", H100_PEAKS["tflops"]),
+                    hbm_gbs=d.get("hbm_gbs", H100_PEAKS["hbm_gbs"]), source="measured (MEASURED_PEAKS.json)")
+    return dict(tflops_sustained=H100_PEAKS["tflops"], tflops_burst=H100_PEAKS["tflops"], hbm_gbs=H100_PEAKS["hbm_gbs"],
+                source="NVIDIA H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -298,9 +311,20 @@ def class_table(prof):
                 "gbs": (v["bytes"] / (v["ms"] / 1e3) / 1e9 if v["ms"] > 0 else 0), "launches": v["launches"]} for k, v in prof.items()}
 
 
-def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup, want_roofline, want_extras, want_parity, clock_sampler=None):
+def dump_outputs(res, out_dir):
+    """The arrays a caller of the timed path receives, as float32 .npy (latents [B,4,h,w], images [B,H,W,3] in 0..255)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in (("latents", res.latents), ("images", res.images)):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
+def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup, want_roofline, want_extras, want_parity, clock_sampler=None,
+                     dump_dir=None, want_cpu=False):
     """Builds the model, runs W warm-ups, times K resident steps and K end-to-end steps (max over ranks, barrier + device
-    sync on both sides), optionally the roofline pass / baselines / shard-parity check. Returns the JSON block (rank 0) or None."""
+    sync on both sides), optionally the roofline pass / baselines / shard-parity check. Returns the JSON block (rank 0) or None.
+    dump_dir: rank 0 writes the last timed resident step's outputs there (dump_outputs)."""
     import torch.distributed as dist
 
     from sdwebui_b200 import lib as L
@@ -340,9 +364,10 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = lib.sdxe_launch_count()
+        last = None
         e0.record()
         for _ in range(k):
-            fn()
+            last = fn()
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -350,14 +375,14 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
             tms = torch.tensor([ms], device=device)
             dist.all_reduce(tms, op=dist.ReduceOp.MAX)
             ms = tms.item()
-        return ms, lib.sdxe_launch_count() - n0
+        return ms, lib.sdxe_launch_count() - n0, last
 
     for _ in range(warmup):
         step_resident()
     step_e2e()
-    # untimed pre-roll: under the 1 kW power cap the SM clock settles ~4-5 % below its cold value over the first seconds
-    # of load; without it the first timed region (`value`) runs on a colder GPU than the second (`e2e`) and the two differ
-    # by drift, not by the host copies (interleaved A/B: 393.1 vs 395.7 ms per batch, tools/profile_pipeline.py)
+    # untimed pre-roll: under a power cap the SM clock settles below its cold value over the first seconds of load;
+    # without it the first timed region (`value`) runs on a colder GPU than the second (`e2e`) and the two differ by
+    # clock drift, not by the host copies
     torch.cuda.synchronize()
     t_roll, n_roll = time.perf_counter(), 0
     while time.perf_counter() - t_roll < PREROLL_S:
@@ -366,8 +391,11 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
         n_roll += 1
     if clock_sampler is not None:
         clock_sampler.start()
-    ms_res, launches = timed(step_resident, steps)
-    ms_e2e, _ = timed(step_e2e, steps)
+    ms_res, launches, last = timed(step_resident, steps)
+    if dump_dir is not None and rank == 0:
+        dump_outputs(last, dump_dir)
+    del last
+    ms_e2e, _, _ = timed(step_e2e, steps)
     clocks = clock_sampler.stop() if clock_sampler is not None else None
 
     # ---- shard parity: rank 0 regenerates the LAST rank's images (N = 1: its own, a second time) and compares pixels
@@ -391,7 +419,7 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
         block = {"metric": f"images/sec {w['name']}", "value": value, "unit": "images/sec", "n_gpus": world, "steps": steps, "warmup": warmup,
                  "ms_per_step": ms_res / steps, "dtype": dtype_name,
                  "config": {"workload": w["name"], "global_batch": B * world, "parallelism": f"dp{world} (image shards, no per-step collective)",
-                            "l2": "working set (>= 1.7 GB weights + activations) >> 126 MB L2: no explicit flush",
+                            "l2": "working set (>= 1.7 GB weights + activations) >> 50 MB L2: no explicit flush",
                             "weights": "random-init, exact architecture", "weight_broadcast_bytes": bcast_bytes,
                             "preroll": f"{n_roll} untimed steps (>= {PREROLL_S:.0f} s of load) after the {warmup} warm-ups: both timed regions at settled clocks"},
                  "e2e": {"value": e2e, "unit": "images/sec", "h2d_bytes_per_step": nbytes(c_host) + nbytes(u_host),
@@ -425,20 +453,10 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
             mm_n = prof_u["gemm"]["launches"] + prof_u["conv3x3"]["launches"]
             achieved = mm_fl / (mm_ms / 1000.0) / 1e12 if mm_ms > 0 else 0.0
             total_u = sum(v["ms"] for v in prof_u.values())
-            traffic, traffic_src = None, None
-            tpath = os.path.join(ROOT, "profiles", "r2_gemm_traffic.json")   # final-tree capture; the round-1 one is the fallback
-            if not os.path.exists(tpath):
-                tpath = os.path.join(ROOT, "profiles", "r1c_gemm_traffic.json")
-            if key == "sd15" and os.path.exists(tpath):  # ncu capture of the same kernel on the same UNet call (SD1.5, 2B = 16)
-                with open(tpath) as f:
-                    tj = json.load(f)
-                traffic = tj["traffic_per_launch_bytes"]
-                traffic_src = tj["source"] + " — a constant from that committed capture, not re-measured by this run"
             block["roofline"] = {
-                "bound": "tensor", "kernel": "sdxe::gemm_kernel (tcgen05 GEMM + implicit-GEMM conv3x3)", "achieved": achieved,
+                "bound": "tensor", "kernel": "sdxe::gemm_kernel (wgmma GEMM + implicit-GEMM conv3x3)", "achieved": achieved,
                 "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops_sustained"],
-                "peak_source": peaks["source"] + ", bf16 sustained (kernel timed inside a long step)", "traffic": traffic,
-                "traffic_unit": "bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum, ncu)", "traffic_source": traffic_src,
+                "peak_source": peaks["source"],
                 "algorithmic_bytes_per_launch": (prof_u["gemm"]["bytes"] + prof_u["conv3x3"]["bytes"]) / max(1, mm_n),
                 "launches_per_unet_call": mm_n, "avg_launch_us": 1000.0 * mm_ms / max(1, mm_n),
                 "share_of_unet_call": mm_ms / total_u if total_u else None,
@@ -455,11 +473,12 @@ def measure_workload(key, dtype_name, rank, world, local, device, steps, warmup,
             block["torch_sdp_gpu"] = torch_sdp_gpu_baseline(key, device, B)
         except Exception as ex:  # noqa: BLE001
             block["torch_sdp_gpu"] = {"unavailable": repr(ex)[:200]}
-        try:
-            cb = cpu_reference_sample(key)
-            block["cpu_baseline"] = {k: cb[k] for k in ("value", "unit", "cores", "kind", "sample")}
-        except Exception as ex:  # noqa: BLE001
-            block["cpu_baseline"] = {"value": None, "unit": "images/sec", "cores": effective_cores(), "kind": "port", "sample": repr(ex)[:200]}
+        if want_cpu:
+            try:
+                cb = cpu_reference_sample(key)
+                block["cpu_baseline"] = {k: cb[k] for k in ("value", "unit", "cores", "kind", "sample")}
+            except Exception as ex:  # noqa: BLE001
+                block["cpu_baseline"] = {"value": None, "unit": "images/sec", "cores": effective_cores(), "kind": "port", "sample": repr(ex)[:200]}
     return block
 
 
@@ -472,8 +491,13 @@ def main():
     ap.add_argument("--config", default=os.environ.get("SDXE_BENCH_CONFIG", "sd15"), choices=["sd15", "sdxl", "c4"],
                     help="the workload reported at the top level of the JSON line (default: BASELINE configs[1])")
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp16"])
-    ap.add_argument("--no-extras", action="store_true", help="skip cpu_baseline / torch-SDP legs")
+    ap.add_argument("--no-extras", action="store_true", help="skip the torch-SDP (and --cpu-baseline) legs")
+    ap.add_argument("--cpu-baseline", action="store_true",
+                    help="also time the CPU reference arm (cpu_baseline) for the headline and sdxl in this run (~100 s of host time)")
     ap.add_argument("--only-headline", action="store_true", help="skip the fp16 / sdxl / c4 blocks")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline's last timed step's outputs (latents, images) to DIR/<name>.npy as float32 "
+                         "(rank 0's shard when --gpus > 1)")
     args = ap.parse_args()
 
     from sdwebui_b200 import parallel as P
@@ -493,7 +517,8 @@ def main():
     extras = not args.no_extras
     warm = max(3, args.warmup)
     sampler = ClockSampler(local) if rank == 0 else None
-    head = measure_workload(args.config, args.dtype, rank, world, local, device, args.steps, warm, True, extras, True, sampler)
+    head = measure_workload(args.config, args.dtype, rank, world, local, device, args.steps, warm, True, extras, True, sampler,
+                            dump_dir=args.dump_outputs, want_cpu=extras and args.cpu_baseline)
     blocks = {}
     if not args.only_headline:
         sub_steps = max(1, min(args.steps, 5))
@@ -503,7 +528,8 @@ def main():
             if key == args.config:
                 continue
             blocks[key] = measure_workload(key, args.dtype, rank, world, local, device, min(sub_steps, 3) if key == "c4" else sub_steps, 3,
-                                           key == "sdxl", extras and key == "sdxl", key == "sdxl")
+                                           key == "sdxl", extras and key == "sdxl", key == "sdxl",
+                                           want_cpu=extras and args.cpu_baseline and key == "sdxl")
     if rank == 0:
         line = dict(head)
         line.update({"higher_is_better": True, "scaling": "weak", "vs_baseline": None, "data": "synthetic"})

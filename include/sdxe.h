@@ -1,4 +1,4 @@
-/* sdxe — B200-native (sm_100a) denoising engine for AUTOMATIC1111/stable-diffusion-webui's hot path.
+/* sdxe — H100-native (sm_90a) denoising engine for AUTOMATIC1111/stable-diffusion-webui's hot path.
  *
  * C-ABI of libsdxe.so. Plain pointers and sizes only; every pointer named "device" is a CUDA device pointer on
  * the current device, `stream` is a cudaStream_t (0 = legacy default stream). No call synchronises the host
@@ -140,7 +140,7 @@ int sdxe_set_plan_cache(sdxe_engine* e, int max_plans, int64_t pool_limit_mb);
 int64_t sdxe_pool_bytes(sdxe_engine* e, int64_t* n_plans);
 
 /* Per-kernel-class timing: while enabled, forward / decode calls run their plan eagerly with a CUDA event pair
- * around every launch on the launching stream. kind: 0 GEMM (tcgen05), 1 conv3x3 implicit GEMM (tcgen05),
+ * around every launch on the launching stream. kind: 0 GEMM (wgmma), 1 conv3x3 implicit GEMM (wgmma),
  * 2 attention, 3 GroupNorm, 4 LayerNorm, 5 other. flops / bytes are ALGORITHMIC totals of the timed launches. */
 int sdxe_profile(sdxe_engine* e, int enable);
 int sdxe_profile_read(sdxe_engine* e, int kind, double* ms, double* flops, double* bytes, int64_t* launches);

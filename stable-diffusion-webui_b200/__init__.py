@@ -1,4 +1,4 @@
-"""stable-diffusion-webui_b200 — a B200-native (sm_100a) denoising engine that plugs in behind
+"""stable-diffusion-webui_b200 — an H100-native (sm_90a) denoising engine that plugs in behind
 AUTOMATIC1111/stable-diffusion-webui's own seams (modules/sd_unet.py, modules/sd_hijack_optimizations.py,
 modules/processing.process_images). Import as `sdwebui_b200` (see ../sdwebui_b200.py).
 

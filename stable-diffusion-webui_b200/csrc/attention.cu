@@ -1,331 +1,226 @@
-// FlashAttention-style softmax(Q K^T * scale) V for sm_100a on tcgen05 + TMEM + TMA.
+// FlashAttention-style softmax(Q K^T * scale) V for sm_90a on wgmma + TMA + mbarrier.
 //
 // Replaces every CrossAttention.forward / AttnBlock.forward variant of the reference
 // (modules/sd_hijack_optimizations.py:180-655: split, Doggettx, InvokeAI, sub-quadratic, xformers, sdp):
 // one kernel for UNet self-attention (Nk = Nq in {4096,1024,256,64}), cross-attention (Nk = 77*k) and the
-// VAE AttnBlock (single head, d = 512, run as two passes over 256-wide halves of V).
+// VAE AttnBlock (single head, d = 512, run as passes over 128-wide slices of V).
 //
 // Inputs are the projection GEMMs' row-major outputs ([B*tokens, 3C] = q|k|v, heads contiguous inside each) seen
 // through 4D tensor maps (d, token, head, batch): a 64-wide slab reaching past the head dim d is zero-filled by TMA,
 // so no padded / transposed per-head copy exists. Output is merged-head [B*Nq, H*d] for the out-projection.
 //
 // CTA = one 128-row query tile of one (batch, head):
-//   warp 0    : TMA producer. Q slabs once (or streamed when d = 512), then K_i / V_i slabs (128 x 64 elements,
-//               16 KB, 128B swizzle) through one in-order ring, in exactly the order the MMA warp consumes them.
-//   warp 1    : tcgen05.mma issuer.  S_i = Q K_i^T -> TMEM (double buffered);  O += P_i V_i -> TMEM.
-//               V is used as an MN-major B operand straight from its natural [kv, dv] layout.
-//   warps 2-9 : online softmax. Each query row is shared by two threads (warps w and w+4 own the same TMEM lane
-//               quarter; one takes key columns 0-63 of the block, the other 64-127) so every scheduler has two
-//               softmax warps to interleave. Row max agreed through a tiny smem exchange + 64-thread named barrier,
-//               partial row sums kept per thread and added at the end. P is written to shared memory in the UMMA
-//               K-major 128B-swizzle layout (double buffered); O is rescaled in TMEM lazily (only when the running
-//               max moved by more than 2^8); final 1/l scaling and store.
+//   warp 8     : TMA producer. Q slabs once (resident), then per 64-key block its K slabs and V slabs (64 x 64
+//                elements, 8 KB, 128B swizzle) through one in-order ring, in exactly the order they are consumed.
+//   warps 0-7  : two warpgroups of 64 query rows each. S = Q K^T with wgmma from shared memory into registers, online
+//                softmax on the accumulator fragment, P converted in registers into the A operand of O += P V
+//                (V read MN-major straight from its natural [kv, dv] layout), final 1/l scaling and store.
 #include "attention.cuh"
+#include "wgmma.cuh"
 #include <algorithm>
-#include <cstdlib>
 
 namespace sdxe {
 
-static constexpr int SLAB_BYTES = 16384;  // 128 rows x 64 x 2 B
-static constexpr int ATT_THREADS = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9 softmax (two warps per TMEM lane quarter)
-static constexpr int TM_S0 = 0, TM_O = 256;  // TMEM columns: S buffers at 0 / 128, O at 256..511
+static constexpr int SLAB_BYTES = 64 * 64 * 2;    // one K or V slab: 64 keys x 64 columns
+static constexpr int Q_SLAB_BYTES = 128 * 64 * 2;  // one Q slab: 128 query rows x 64 columns
+static constexpr int ATT_THREADS = 288;            // warpgroups 0-1: MMA + softmax, warp 8: TMA producer
+static constexpr int CONSUMER_WARPS = 8;
+static constexpr int KV_BLOCK = 64;
+static constexpr int SMEM_BUDGET = 227 * 1024;
 
-template <bool BF16>
+template <bool BF16, int NVS>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_constant__ AttnArgs a) {
   using T = T16<BF16>;
-  using TT = typename T::type;
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t pad = ((raw + 1023u) & ~1023u) - raw;
-  uint8_t* smem = smem_raw + pad;
-  const uint32_t sbase = raw + pad;
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
   const int NS = a.num_slots;
-  const int q_slabs = a.q_resident ? a.dqk_slabs : 0;
   const uint32_t sQ = sbase;
-  const uint32_t sRing = sQ + q_slabs * SLAB_BYTES;
-  const uint32_t sP = sRing + NS * SLAB_BYTES;   // two P tiles (double buffered), 2 slabs each
-  const uint32_t bar_base = sP + 4 * SLAB_BYTES;
+  const uint32_t sRing = sQ + a.dqk_slabs * Q_SLAB_BYTES;
+  const uint32_t bar_base = sRing + NS * SLAB_BYTES;
   auto slot_full = [&](int s) { return bar_base + 8u * s; };
   auto slot_empty = [&](int s) { return bar_base + 8u * (NS + s); };
   const uint32_t q_full = bar_base + 8u * (2 * NS);
-  auto s_full = [&](int i) { return bar_base + 8u * (2 * NS + 1 + i); };
-  // per-P-buffer barriers: a waiter is never more than one phase behind on any of them
-  auto p_ready = [&](int i) { return bar_base + 8u * (2 * NS + 3 + i); };
-  auto pv_done = [&](int i) { return bar_base + 8u * (2 * NS + 5 + i); };
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + (bar_base - sbase) + 8 * (2 * NS + 7));
-  float* xch = reinterpret_cast<float*>(smem + (bar_base - sbase) + 8 * (2 * NS + 7) + 16);  // [2 buf][2 halves][128 rows]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
   const int hb_b = bh / a.H, hb_h = bh - hb_b * a.H;  // (batch, head) coordinates of the 4D per-head tensor maps
-  const int nblk = (a.Nk + 127) / 128;
+  const int nblk = (a.Nk + KV_BLOCK - 1) / KV_BLOCK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) { mbar_init(slot_full(s), 1); mbar_init(slot_empty(s), 1); }
+    for (int s = 0; s < NS; ++s) { mbar_init(slot_full(s), 1); mbar_init(slot_empty(s), CONSUMER_WARPS); }
     mbar_init(q_full, 1);
-    mbar_init(s_full(0), 1);
-    mbar_init(s_full(1), 1);
-    mbar_init(p_ready(0), 8);
-    mbar_init(p_ready(1), 8);
-    mbar_init(pv_done(0), 1);
-    mbar_init(pv_done(1), 1);
     fence_mbar_init();
     tma_prefetch_desc(&a.tmQ);
     tma_prefetch_desc(&a.tmK);
     tma_prefetch_desc(&a.tmV);
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_ptr_smem), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();  // q / k / v of the producing GEMM are complete; the output buffer is free
 
-  if (warp == 0) {
-    // ---------------------------------------------------------------- producer
-    // converged warp, elected issue (see gemm.cu)
-    {
-      if (a.q_resident && elect_one()) {
-        mbar_expect_tx(q_full, a.dqk_slabs * SLAB_BYTES);
-        for (int c = 0; c < a.dqk_slabs; ++c) tma_load_4d(sQ + c * SLAB_BYTES, &a.tmQ, q_full, c * 64, q0, hb_h, hb_b);
+  if (warp == CONSUMER_WARPS) {
+    // ---------------------------------------------------------------- producer (converged warp, elected issue)
+    if (elect_one()) {
+      mbar_expect_tx(q_full, a.dqk_slabs * Q_SLAB_BYTES);
+      for (int c = 0; c < a.dqk_slabs; ++c) tma_load_4d(sQ + c * Q_SLAB_BYTES, &a.tmQ, q_full, c * 64, q0, hb_h, hb_b);
+    }
+    __syncwarp();
+    int slot = 0;
+    uint32_t phase = 0;
+    auto push = [&](const CUtensorMap* tm, int c0, int r0) {
+      mbar_wait(slot_empty(slot), phase ^ 1u);
+      if (elect_one()) {
+        mbar_expect_tx(slot_full(slot), SLAB_BYTES);
+        tma_load_4d(sRing + slot * SLAB_BYTES, tm, slot_full(slot), c0, r0, hb_h, hb_b);
       }
       __syncwarp();
-      int slot = 0;
-      uint32_t phase = 0;
-      auto push = [&](const CUtensorMap* tm, int c0, int r0) {
-        mbar_wait(slot_empty(slot), phase ^ 1u);
-        if (elect_one()) {
-          mbar_expect_tx(slot_full(slot), SLAB_BYTES);
-          tma_load_4d(sRing + slot * SLAB_BYTES, tm, slot_full(slot), c0, r0, hb_h, hb_b);
-        }
-        __syncwarp();
-        if (++slot == NS) { slot = 0; phase ^= 1u; }
-      };
-      for (int i = 0; i <= nblk; ++i) {
-        if (i < nblk) {
-          for (int c = 0; c < a.dqk_slabs; ++c) {
-            if (!a.q_resident) push(&a.tmQ, c * 64, q0);
-            push(&a.tmK, c * 64, i * 128);
-          }
-        }
-        if (i >= 1)
-          for (int vs = 0; vs < a.dv_slabs; ++vs) push(&a.tmV, vs * 64, (i - 1) * 128);
-      }
+      if (++slot == NS) { slot = 0; phase ^= 1u; }
+    };
+    for (int j = 0; j < nblk; ++j) {
+      for (int c = 0; c < a.dqk_slabs; ++c) push(&a.tmK, c * 64, j * KV_BLOCK);
+      for (int vs = 0; vs < NVS; ++vs) push(&a.tmV, vs * 64, j * KV_BLOCK);
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (converged warp, elected issue)
-    {
-      const uint32_t idesc_s = umma_idesc(BF16 ? 1 : 0, 128, 128, 0, 0);
-      const uint32_t idesc_pv = umma_idesc(BF16 ? 1 : 0, 128, 64, 0, 1);
-      // zero-padded tails are skipped: fewer K steps on the last Q/K slab, narrower N on the last V slab
-      const int ksteps_last = (a.dqk - (a.dqk_slabs - 1) * 64 + 15) / 16;
-      const int n_last = (a.dv - (a.dv_slabs - 1) * 64 + 15) / 16 * 16;
-      const uint32_t idesc_pv_last = umma_idesc(BF16 ? 1 : 0, 128, n_last, 0, 1);
-      int slot = 0;
-      uint32_t phase = 0;
-      auto pop = [&]() -> uint32_t {  // wait for the next slab in ring order, return its smem address
-        mbar_wait(slot_full(slot), phase);
-        return sRing + slot * SLAB_BYTES;
-      };
-      auto release = [&]() {  // slab is freed when the MMAs issued so far complete (caller is the elected lane)
-        tc_commit(slot_empty(slot));
-      };
-      auto advance = [&]() { if (++slot == NS) { slot = 0; phase ^= 1u; } };
-      if (a.q_resident) mbar_wait(q_full, 0);
-      for (int i = 0; i <= nblk; ++i) {
-        if (i < nblk) {
-          const uint32_t d_s = tmem_base + TM_S0 + (uint32_t)((i & 1) * 128);
-          for (int c = 0; c < a.dqk_slabs; ++c) {
-            uint32_t q_addr;
-            int q_slot_held = 0;
-            if (a.q_resident) q_addr = sQ + c * SLAB_BYTES;
-            else { q_addr = pop(); q_slot_held = 1; }
-            // when Q is streamed its slab must stay valid until the K slab's MMAs are issued:
-            // advance manually past it, release both afterwards (commit order == ring order).
-            int q_slot = slot;
-            uint32_t q_phase = phase;
-            if (q_slot_held) { if (++slot == NS) { slot = 0; phase ^= 1u; } }
-            const uint32_t k_addr = pop();
-            tc_fence_after();
-            const uint64_t qd = umma_desc_sw128(q_addr, 16, 1024);
-            const uint64_t kd = umma_desc_sw128(k_addr, 16, 1024);
-            const int ks = (c == a.dqk_slabs - 1) ? ksteps_last : 4;
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                if (k < ks) tc_mma_f16(d_s, qd + 2 * k, kd + 2 * k, idesc_s, (c | k) != 0 ? 1u : 0u);
-              if (q_slot_held) tc_commit(slot_empty(q_slot));
-              release();
-              if (c == a.dqk_slabs - 1) tc_commit(s_full(i & 1));
-            }
-            __syncwarp();
-            (void)q_phase;
-            advance();
-          }
-        }
-        if (i >= 1) {
-          const int j = i - 1;  // O += P_j V_j
-          mbar_wait(p_ready(j & 1), (uint32_t)((j >> 1) & 1));
-          tc_fence_after();
-          const uint32_t sPj = sP + (uint32_t)(j & 1) * 2 * SLAB_BYTES;
-          const uint64_t pd0 = umma_desc_sw128(sPj, 16, 1024), pd1 = umma_desc_sw128(sPj + SLAB_BYTES, 16, 1024);
-          for (int vs = 0; vs < a.dv_slabs; ++vs) {
-            const uint32_t v_addr = pop();
-            tc_fence_after();
-            const uint32_t d_o = tmem_base + TM_O + (uint32_t)(vs * 64);
-            const uint64_t vd = umma_desc_sw128(v_addr, SLAB_BYTES, 1024);
-            const uint32_t id = (vs == a.dv_slabs - 1) ? idesc_pv_last : idesc_pv;
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k)  // +16 key rows: +128 in V's addr>>4 field, +2 in P's
-                tc_mma_f16(d_o, (k < 4 ? pd0 : pd1) + 2 * (k & 3), vd + 128 * k, id, (j | k) != 0 ? 1u : 0u);
-              release();
-              if (vs == a.dv_slabs - 1) tc_commit(pv_done(j & 1));
-            }
-            __syncwarp();
-            advance();
-          }
-        }
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- softmax / epilogue
-    const int quarter = warp & 3;            // TMEM lane quarter (warps w and w+4 share it)
-    const int half = (warp - 2) >> 2;        // which 64 key columns of each block this thread owns
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const float sl2 = a.scale_log2;
-    const uint32_t pair_bar = 1u + (uint32_t)quarter;  // named barrier of the two warps sharing these 32 rows
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int i = 0; i < nblk; ++i) {
-      mbar_wait(s_full(i & 1), (uint32_t)((i >> 1) & 1));
-      tc_fence_after();
-      const uint32_t t_s = tmem_base + TM_S0 + (uint32_t)((i & 1) * 128) + lane_base + (uint32_t)(half * 64);
-      const int kv0 = i * 128 + half * 64;
-      uint32_t sreg[64];
-      tmem_ld32(t_s, sreg);
-      tmem_ld32(t_s + 32, sreg + 32);
-      tc_wait_ld();
-      if (kv0 + 64 > a.Nk) {  // only the tail of the last block has invalid key columns
-#pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (kv0 + j >= a.Nk) sreg[j] = 0xff800000u;  // -inf
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 64; j += 4) {
-        mx0 = fmaxf(mx0, __uint_as_float(sreg[j]));
-        mx1 = fmaxf(mx1, __uint_as_float(sreg[j + 1]));
-        mx2 = fmaxf(mx2, __uint_as_float(sreg[j + 2]));
-        mx3 = fmaxf(mx3, __uint_as_float(sreg[j + 3]));
-      }
-      float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      // agree on the row max with the thread that owns the other 64 columns
-      float* xb = xch + (i & 1) * 256;
-      xb[half * 128 + row] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      mx = fmaxf(mx, xb[(half ^ 1) * 128 + row]);
-      // lazy rescale: keep a stale running max until it is off by more than 2^8 (p stays <= 256, exact after 1/l)
-      const float m_cand = fmaxf(m_run, mx);
-      const bool need = (m_cand - m_run) * sl2 > 8.f;  // first block: +inf > 8
-      if (__any_sync(0xffffffffu, need)) {             // identical decision in both warps of the pair
-        const float alpha = ex2_approx((m_run - m_cand) * sl2);  // first block: 0
-        if (i >= 1) {
-          mbar_wait(pv_done((i - 1) & 1), (uint32_t)(((i - 1) >> 1) & 1));  // O holds every block < i
-          tc_fence_after();
-          for (int c = half * a.dv_slabs; c < (half + 1) * a.dv_slabs; ++c) {  // each half rescales its O columns
-            uint32_t r[32];
-            const uint32_t t_o = tmem_base + TM_O + lane_base + c * 32;
-            tmem_ld32(t_o, r);
-            tc_wait_ld();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) * alpha);
-            tmem_st32(t_o, r);
-          }
-          tc_wait_st();
-        }
-        l_run *= alpha;
-        m_run = m_cand;
-      }
-      const float mb = m_run * sl2;
-      if (i >= 2) mbar_wait(pv_done(i & 1), (uint32_t)(((i >> 1) + 1) & 1));  // P buffer (i & 1) free: PV(i-2) done
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-      // this half's 64 columns = K-major 128B-swizzle atom `half` of P buffer (i & 1)
-      const uint32_t p_row = sP + (uint32_t)(i & 1) * 2 * SLAB_BYTES + (uint32_t)half * SLAB_BYTES + row * 128;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float p0 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 0]), sl2, -mb));
-        const float p1 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 1]), sl2, -mb));
-        const float p2 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 2]), sl2, -mb));
-        const float p3 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 3]), sl2, -mb));
-        const float p4 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 4]), sl2, -mb));
-        const float p5 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 5]), sl2, -mb));
-        const float p6 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 6]), sl2, -mb));
-        const float p7 = ex2_approx(fmaf(__uint_as_float(sreg[q * 8 + 7]), sl2, -mb));
-        s0 += p0 + p1; s1 += p2 + p3; s2 += p4 + p5; s3 += p6 + p7;
-        const uint32_t chunk = (uint32_t)q ^ (uint32_t)(row & 7);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(p_row + chunk * 16), "r"(T::pack(p0, p1)),
-                     "r"(T::pack(p2, p3)), "r"(T::pack(p4, p5)), "r"(T::pack(p6, p7))
-                     : "memory");
-      }
-      l_run += (s0 + s1) + (s2 + s3);
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready(i & 1));
-    }
-    // ---- epilogue: O / l -> out[b, q, h*dv + j]; the row sum is the sum of the two halves' partial sums
-    {
-      float* xb = xch + (nblk & 1) * 256;
-      xb[half * 128 + row] = l_run;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      l_run += xb[(half ^ 1) * 128 + row];
-    }
-    mbar_wait(pv_done((nblk - 1) & 1), (uint32_t)(((nblk - 1) >> 1) & 1));
-    tc_fence_after();
-    const int q = q0 + row;
-    const float inv_l = 1.f / l_run;
-    const int b = bh / a.H, h = bh - b * a.H;
-    TT* orow = reinterpret_cast<TT*>(a.out) + ((size_t)b * a.Nq + q) * a.ldo + a.out_col0 + h * a.dv;
-    for (int c = half * a.dv_slabs; c < (half + 1) * a.dv_slabs; ++c) {
-      if (c * 32 >= a.dv) break;
-      uint32_t r[32];
-      tmem_ld32(tmem_base + TM_O + lane_base + c * 32, r);
-      tc_wait_ld();
-      if (q < a.Nq) {
-#pragma unroll
-        for (int g = 0; g < 32; g += 8) {
-          if (c * 32 + g + 8 <= a.dv) {
-            uint4 u;
-            u.x = T::pack(__uint_as_float(r[g + 0]) * inv_l, __uint_as_float(r[g + 1]) * inv_l);
-            u.y = T::pack(__uint_as_float(r[g + 2]) * inv_l, __uint_as_float(r[g + 3]) * inv_l);
-            u.z = T::pack(__uint_as_float(r[g + 4]) * inv_l, __uint_as_float(r[g + 5]) * inv_l);
-            u.w = T::pack(__uint_as_float(r[g + 6]) * inv_l, __uint_as_float(r[g + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c * 32 + g) = u;
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ------------------------------------------------------------------ MMA + softmax warpgroups
+  // Accumulator fragment of wgmma m64n64 (per warp 16 rows): x[4 i + 2 h + e] is row (lane / 4 + 8 h) of the warp's
+  // band, column 8 i + 2 (lane % 4) + e.
+  const int wg = warp >> 2;
+  const int band = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const float sl2 = a.scale_log2;
+  const uint64_t qdesc0 = gmma_desc_sw128(sQ + (uint32_t)wg * (64 * 128), 16, 1024);
+  float o[NVS][32];
+#pragma unroll
+  for (int vs = 0; vs < NVS; ++vs)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[vs][i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  int slot = 0;
+  uint32_t phase = 0;
+  auto advance = [&]() { if (++slot == NS) { slot = 0; phase ^= 1u; } };
+  auto release_from = [&](int first, int count) {  // slots first .. first + count - 1 (ring order) may be refilled
+    if (lane == 0)
+      for (int t = 0, s = first; t < count; ++t, s = (s + 1 == NS) ? 0 : s + 1) mbar_arrive(slot_empty(s));
+  };
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < nblk; ++j) {
+    // ---- S = Q K_j^T
+    float s[32];
+    const int k_first = slot;
+    for (int c = 0; c < a.dqk_slabs; ++c) {
+      mbar_wait(slot_full(slot), phase);
+      wgmma_fence();
+      const uint64_t kd = gmma_desc_sw128(sRing + slot * SLAB_BYTES, 16, 1024);
+      const uint64_t qd = qdesc0 + (uint64_t)(c * (Q_SLAB_BYTES >> 4));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<64, BF16>(s, qd + 2 * k, kd + 2 * k, (c | k) != 0);
+      wgmma_commit();
+      advance();
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(s[i]);
+    release_from(k_first, a.dqk_slabs);
+
+    // ---- online softmax on the fragment (a row's 64 columns live in the four threads of a quad)
+    const int kv0 = j * KV_BLOCK;
+    if (kv0 + KV_BLOCK > a.Nk) {  // only the last block has invalid key columns
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kv0 + 8 * i + cq + e >= a.Nk) { s[4 * i + e] = -INFINITY; s[4 * i + 2 + e] = -INFINITY; }
+    }
+    float mb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);  // finite: every block holds at least one valid key
+      const float alpha = ex2_approx((m_run[h] - m_new) * sl2);  // first block: 2^-inf = 0
+      l_run[h] *= alpha;
+#pragma unroll
+      for (int vs = 0; vs < NVS; ++vs)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { o[vs][4 * i + 2 * h] *= alpha; o[vs][4 * i + 2 * h + 1] *= alpha; }
+      m_run[h] = m_new;
+      mb[h] = m_new * sl2;
+    }
+    // P in the A-operand fragment of m64nNk16: key step kk uses column blocks 2 kk (regs 0, 1) and 2 kk + 1 (regs 2, 3)
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      float p[4];
+#pragma unroll
+      for (int t = 0; t < 4; ++t) p[t] = ex2_approx(fmaf(s[4 * i + t], sl2, -mb[t >> 1]));
+      l_run[0] += p[0] + p[1];
+      l_run[1] += p[2] + p[3];
+      pa[i >> 1][(i & 1) * 2 + 0] = T::pack(p[0], p[1]);
+      pa[i >> 1][(i & 1) * 2 + 1] = T::pack(p[2], p[3]);
+    }
+
+    // ---- O += P V_j
+    const int v_first = slot;
+#pragma unroll
+    for (int vs = 0; vs < NVS; ++vs) {
+      mbar_wait(slot_full(slot), phase);
+      wgmma_fence();
+      const uint64_t vd = gmma_desc_sw128(sRing + slot * SLAB_BYTES, SLAB_BYTES, 1024);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs_tb<64, BF16>(o[vs], pa[kk], vd + 128 * kk, 1);  // +16 key rows = +2048 B
+      wgmma_commit();
+      advance();
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int vs = 0; vs < NVS; ++vs)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) reg_fence(o[vs][i]);
+    release_from(v_first, NVS);
   }
+
+  // ---- epilogue: O / l -> out[b, q, out_col0 + h * out_hstride + j]
+  using TT = typename T::type;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.f / l;
+    const int q = q0 + wg * 64 + band + 8 * h;
+    if (q >= a.Nq) continue;
+    TT* orow = reinterpret_cast<TT*>(a.out) + ((size_t)hb_b * a.Nq + q) * a.ldo + a.out_col0 + hb_h * a.out_hstride;
+#pragma unroll
+    for (int vs = 0; vs < NVS; ++vs)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int col = vs * 64 + 8 * i + cq;  // even, dv a multiple of 8: col + 1 is valid with col
+        if (col < a.dv)
+          *reinterpret_cast<uint32_t*>(orow + col) = T::pack(o[vs][4 * i + 2 * h] * inv_l, o[vs][4 * i + 2 * h + 1] * inv_l);
+      }
+  }
+}
+
+typedef void (*AttnKernel)(const AttnArgs);
+static AttnKernel attention_variant(bool bf16, int nvs) {
+  if (bf16) return nvs == 1 ? attention_kernel<true, 1> : attention_kernel<true, 2>;
+  return nvs == 1 ? attention_kernel<false, 1> : attention_kernel<false, 2>;
 }
 
 int attention_init() {
   static bool done = false;
   if (!done) {
-    SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    if (attention2_init() != 0) return -1;
-    if (attentionx_init() != 0) return -1;
+    for (int b = 0; b < 2; ++b)
+      for (int nvs = 1; nvs <= 2; ++nvs)
+        SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_variant(b != 0, nvs), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET));
     done = true;
   }
   return 0;
@@ -333,30 +228,19 @@ int attention_init() {
 
 int attention_launch(const AttnArgs& a_in, bool bf16, cudaStream_t stream) {
   AttnArgs a = a_in;
-  {
-    // SDXE_ATTN: 2 = attention2 (two Q tiles, an MMA issuer per tile, 16 softmax warps) where eligible [default],
-    //            1 = this file's kernel only
-    static int mode = -1;
-    if (mode < 0) { const char* e = getenv("SDXE_ATTN"); mode = e ? atoi(e) : 2; }
-    static int usex = -1;  // SDXE_ATTNX=0: keep short-KV (cross-) attention on the general kernels
-    if (usex < 0) { const char* e = getenv("SDXE_ATTNX"); usex = e ? atoi(e) : 1; }
-    if (usex && attentionx_eligible(a)) return attentionx_launch(a, bf16, stream);
-    if (mode >= 2 && attention2_eligible(a)) return attention2_launch(a, bf16, stream);
-  }
-  if (a.dv_slabs < 1 || a.dv_slabs > 4 || a.dqk_slabs < 1 || a.dqk_slabs > 8 || a.dv % 8 != 0 || a.dv > a.dv_slabs * 64) {
+  if (a.dv_slabs < 1 || a.dv_slabs * 64 > ATTN_MAX_DV || a.dqk_slabs < 1 || a.dqk_slabs > 8 || a.dv % 8 != 0 ||
+      a.dv > a.dv_slabs * 64) {
     set_last_error(__FILE__, __LINE__, "attention: unsupported head size");
     return -1;
   }
-  a.q_resident = a.dqk_slabs <= 3 ? 1 : 0;
-  const int q_slabs = a.q_resident ? a.dqk_slabs : 0;
-  const int budget = (224 * 1024 - 2048) / SLAB_BYTES;  // slabs that fit beside barriers + alignment slack
-  a.num_slots = std::min(10, budget - 4 - q_slabs);
-  if (a.num_slots < 2) { set_last_error(__FILE__, __LINE__, "attention: smem"); return -1; }
-  const size_t smem = (size_t)(q_slabs + a.num_slots + 4) * SLAB_BYTES + 8 * (2 * a.num_slots + 7) + 16 + 2048 + 1024;
-  auto kern = bf16 ? attention_kernel<true> : attention_kernel<false>;
+  const size_t fixed = 1024 /*alignment*/ + (size_t)a.dqk_slabs * Q_SLAB_BYTES + 8;
+  // every K slab of a block stays resident until the block's S is complete, so the ring holds at least dqk_slabs
+  a.num_slots = (int)std::min<size_t>(16, (SMEM_BUDGET - fixed) / (SLAB_BYTES + 16));
+  if (a.num_slots < std::max(2, a.dqk_slabs)) { set_last_error(__FILE__, __LINE__, "attention: smem"); return -1; }
+  const size_t smem = fixed + (size_t)a.num_slots * (SLAB_BYTES + 16);
   if (attention_init() != 0) return -1;
   dim3 grid((a.Nq + 127) / 128, a.B * a.H);
-  SDXE_CUDA_CHECK(launch_k(kern, grid, dim3(ATT_THREADS), smem, stream, a));
+  SDXE_CUDA_CHECK(launch_k(attention_variant(bf16, a.dv_slabs), grid, dim3(ATT_THREADS), smem, stream, a));
   return 0;
 }
 

@@ -1,4 +1,4 @@
-// Argument block of the tcgen05 flash-attention kernel (attention.cu).
+// Argument block of the wgmma flash-attention kernel (attention.cu).
 #pragma once
 #include "common.cuh"
 
@@ -6,33 +6,28 @@ namespace sdxe {
 
 struct alignas(64) AttnArgs {
   // 4D per-head views (common.cuh make_tmap_heads): {d (true head dim: boxes reaching past it are zero-filled), token,
-  // head, batch}, box 64 x 128 x 1 x 1, 128B swizzle
+  // head, batch}, 128B swizzle. Box 64 x 128 for Q, 64 x 64 for K and V.
   CUtensorMap tmQ;
   CUtensorMap tmK;
   CUtensorMap tmV;
   int B, H, Nq, Nk;
   int dqk_slabs;    // dqk_pad / 64  (1..8)
-  int dv_slabs;     // dv_pad / 64   (1..4)
-  int dv;           // valid value columns per head that are stored (multiple of 8)
+  int dv_slabs;     // value columns of this pass / 64, rounded up (1..2); wider heads run in several passes
+  int dv;           // valid value columns of this pass that are stored (multiple of 8)
   int dqk;          // valid q/k columns (<= dqk_slabs * 64); columns beyond are zero padding
-  int q_resident;   // set by the launcher
   int num_slots;    // set by the launcher
   float scale_log2; // softmax scale * log2(e)
-  void* out;        // [B*Nq, ldo] 16-bit; head h writes columns out_col0 + h*dv ...
+  void* out;        // [B*Nq, ldo] 16-bit; head h writes columns out_col0 + h*out_hstride ...
   int ldo;
   int out_col0;
-  unsigned long long* trace;  // timeline of CTA (0,0), only in builds with -DSDXE_ATT_TRACE=1; null otherwise
+  int out_hstride;
 };
+
+static constexpr int ATTN_Q_BOX_ROWS = 128;
+static constexpr int ATTN_KV_BOX_ROWS = 64;
+static constexpr int ATTN_MAX_DV = 128;  // value columns per pass
 
 int attention_launch(const AttnArgs& a, bool bf16, cudaStream_t stream);
 int attention_init();
-// two-query-tile variant (attention2.cu), used automatically by attention_launch when eligible
-bool attention2_eligible(const AttnArgs& a);
-int attention2_launch(const AttnArgs& a, bool bf16, cudaStream_t stream);
-int attention2_init();
-// persistent, software-pipelined short-KV (cross-) attention: Nk <= 128, head dim <= 64 (attention_x.cu)
-bool attentionx_eligible(const AttnArgs& a);
-int attentionx_launch(const AttnArgs& a, bool bf16, cudaStream_t stream);
-int attentionx_init();
 
 }  // namespace sdxe

@@ -23,17 +23,17 @@ int sdxe_attention(const void* q, const void* k, const void* v, void* out, int B
   if (!is16(dtype) || D % 8 != 0 || D > 512 || D <= 0) { set_last_error(__FILE__, __LINE__, "sdxe_attention: dtype/D"); return -2; }
   const bool bf16 = dtype == SDXE_BF16;
   const int Dpad = (D + 63) / 64 * 64;
-  // value dim is processed in passes of at most 256 columns (TMEM: 2 x 128 S columns + 256 O columns)
+  // value dim is processed in passes of at most ATTN_MAX_DV columns (the O accumulator lives in registers)
   int rc = 0;
-  for (int v0 = 0; v0 < D && rc == 0; v0 += 256) {
-    const int dv = std::min(256, D - v0);
+  for (int v0 = 0; v0 < D && rc == 0; v0 += ATTN_MAX_DV) {
+    const int dv = std::min(ATTN_MAX_DV, D - v0);
     AttnArgs a;
     memset(&a, 0, sizeof(a));
     // [B, H, N, D] contiguous seen as (d, token, head, batch); boxes reaching past D are zero-filled by TMA
-    if (make_tmap_heads(&a.tmQ, q, D, Nq, H, B, D, (int64_t)Nq * D, (int64_t)H * Nq * D, 128)) return -1;
-    if (make_tmap_heads(&a.tmK, k, D, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, 128)) return -1;
+    if (make_tmap_heads(&a.tmQ, q, D, Nq, H, B, D, (int64_t)Nq * D, (int64_t)H * Nq * D, ATTN_Q_BOX_ROWS)) return -1;
+    if (make_tmap_heads(&a.tmK, k, D, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, ATTN_KV_BOX_ROWS)) return -1;
     const int dvpad = (dv + 63) / 64 * 64;
-    if (make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, 128)) return -1;
+    if (make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, ATTN_KV_BOX_ROWS)) return -1;
     a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk;
     a.dqk_slabs = Dpad / 64;
     a.dv_slabs = dvpad / 64;
@@ -43,8 +43,7 @@ int sdxe_attention(const void* q, const void* k, const void* v, void* out, int B
     a.out = out;
     a.ldo = H * D;
     a.out_col0 = v0;
-    // heads are interleaved in the output as h*D + j: with a split value dim the head stride is still D
-    if (D > 256 && H != 1) { set_last_error(__FILE__, __LINE__, "sdxe_attention: D > 256 needs H == 1"); rc = -2; break; }
+    a.out_hstride = D;  // heads are interleaved in the output as h*D + j, whatever slice of the value dim a pass covers
     rc = attention_launch(a, bf16, stream);
     count_launch();
   }

@@ -1,6 +1,5 @@
-// sm_100a device primitives shared by every kernel of the denoising engine:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / st / commit),
-// UMMA shared-memory + instruction descriptors, and 16-bit pack helpers.
+// sm_90a device primitives shared by every kernel of the denoising engine:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and shared-memory descriptors, and 16-bit pack helpers.
 // Everything here is inline PTX; nothing is borrowed from a library at run time.
 #pragma once
 #include <cuda.h>
@@ -68,17 +67,15 @@ SDXE_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
     if ((it & 0x3ff) == 0x3ff) {
       uint64_t now = global_timer_ns();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000ull) {  // 4 s
-        printf("sdxe: mbarrier watchdog block(%d,%d,%d) thread %d bar 0x%x parity %u\n", blockIdx.x,
-               blockIdx.y, blockIdx.z, threadIdx.x, bar, parity);
-        __trap();
-      }
+      // 4 s. No printf: mbar_wait serves the wgmma kernels, and any function call in a kernel makes ptxas serialise all
+      // of its wgmma (warning C7510, reported for every GEMM variant when the diagnostic printf was here)
+      else if (now - t0 > 4000000000ull) __trap();
     }
   }
 }
 
 // Programmatic dependent launch (PDL). A kernel launched through launch_k() may start while its predecessor in the
-// stream is still draining: everything before pdl_wait() (smem carve-up, mbarrier init, TMEM allocation, tensor-map
+// stream is still draining: everything before pdl_wait() (smem carve-up, mbarrier init, tensor-map
 // prefetch) overlaps the predecessor's tail; pdl_wait() returns once the predecessor grid has completed and its writes
 // are visible, so NO global memory may be read or written before it. pdl_launch_dependents() lets the successor
 // begin launching once every CTA of this grid has started. Both are no-ops for a normally launched kernel.
@@ -98,7 +95,7 @@ SDXE_DEVINL bool mbar_test(uint32_t bar, uint32_t parity) {
   return done != 0;
 }
 
-// generic-proxy smem writes -> visible to async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to async proxy (TMA stores / wgmma operand reads)
 SDXE_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
@@ -143,178 +140,32 @@ SDXE_DEVINL void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.r
 SDXE_DEVINL void bulk_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }    // all but the newest group
 SDXE_DEVINL void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }            // writes done
 
-// multicast variant: the box lands at the same smem offset in every CTA of `mask`, each CTA's mbarrier (same offset)
-// receives the complete_tx for the bytes written into it
-SDXE_DEVINL void tma_load_2d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// ---- CTA-pair (cta_group::2) forms. The mbarrier operand of a pair TMA load is a shared::cluster address whose
-// "peer bit" (bit 24) selects the CTA of the pair; clearing it makes both CTAs' loads signal the LEADER's barrier
-// (cute/arch/copy_sm100_tma.hpp: Sm100MmaPeerBitMask).
-static constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-SDXE_DEVINL void tma2_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-SDXE_DEVINL void tma2_load_4d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-SDXE_DEVINL void mbar_arrive_remote(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"
-      ::"r"(bar), "r"(cta)
-      : "memory");
-}
-SDXE_DEVINL uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-SDXE_DEVINL void cluster_sync_all() {  // every thread of every CTA of the cluster
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
+// ---------------------------------------------------------------------------------------------
+// wgmma (sm_90a warpgroup MMA): fences and group completion. The MMA wrappers themselves are in wgmma.cuh.
+// ---------------------------------------------------------------------------------------------
+// orders this thread's register writes (accumulators, A fragments) before the next wgmma reads them
+SDXE_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SDXE_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> SDXE_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across wgmma issue / wait
+SDXE_DEVINL void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, MMA, ld/st
-// ---------------------------------------------------------------------------------------------
-SDXE_DEVINL void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {  // whole warp, ncols pow2 >= 32
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-SDXE_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-SDXE_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SDXE_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// All previously issued tcgen05.mma of this thread arrive on `bar` when complete.
-SDXE_DEVINL void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of `mask` (smem slot shared through TMA multicast)
-SDXE_DEVINL void tc_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// ---- cta_group::2: one MMA spans the CTA pair (M = 256: 128 accumulator rows in each CTA's TMEM; A from each CTA's
-// own smem, B rows split half / half across the two CTAs' smem). Issued by the leader CTA only.
-SDXE_DEVINL void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-SDXE_DEVINL void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-SDXE_DEVINL void tc2_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-SDXE_DEVINL void tc2_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], 16-bit inputs, fp32 accumulate.
-SDXE_DEVINL void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with the A operand read from tensor memory (TS form): A = [128 rows (lanes) x 16 k] 16-bit, two elements per 32-bit
-// column (k even in the low half), 8 columns per K = 16 step
-SDXE_DEVINL void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-SDXE_DEVINL void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-SDXE_DEVINL void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives row (lane base + i), 32 consecutive columns.
-SDXE_DEVINL void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-SDXE_DEVINL void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-SDXE_DEVINL void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp, restated).
-//
-// Shared-memory matrix descriptor (64 bit):
+// wgmma shared-memory matrix descriptor (64 bit), 128B swizzle:
 //   [0,14)  start address >> 4          [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4 [46,48) version = 1 (Blackwell)
-//   [49,52) base offset = 0             [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
+//   [32,46) stride-dim byte offset >> 4 [49,52) base offset = 0      [62,64) layout: 1 = 128B swizzle
 //
-// K-major, 128B swizzle, 16-bit elements (our A/B tiles: rows of 64 elements = 128 bytes, as TMA
-// writes them): 8-row groups are 1024 B apart -> SBO = 1024; LBO unused (1).
-// MN-major, 128B swizzle (our V slabs: [kv rows][64 dv] with 128-byte rows): along K 8-row groups
-// are 1024 B apart -> SBO = 1024; LBO = distance between 64-element MN chunks (slab size).
+// K-major (our A/B tiles: rows of 64 elements = 128 bytes, as TMA writes them): 8-row groups are 1024 B apart ->
+// SBO = 1024; LBO unused (1). A K step of 16 elements (32 bytes, inside the swizzle atom) adds 2 to the address field.
+// MN-major (V slabs: [kv rows][64 dv] with 128-byte rows, read transposed): 8-row groups along K are 1024 B apart ->
+// SBO = 1024; LBO = distance between 64-element MN chunks (one slab here, so unused). 16 K rows add 128.
 // ---------------------------------------------------------------------------------------------
-SDXE_DEVINL uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+SDXE_DEVINL uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16 (fp16 or bf16 inputs, fp32 accumulate).
-//   [4,6) c fmt (1 = f32)  [7,10) a fmt  [10,13) b fmt (0 = f16, 1 = bf16)
-//   [15] a major (0 = K)   [16] b major (0 = K, 1 = MN)   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ inline uint32_t umma_idesc(int bf16, int M, int N, int a_mn_major, int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (uint32_t)(bf16 ? 1 : 0) << 7;
-  d |= (uint32_t)(bf16 ? 1 : 0) << 10;
-  d |= (uint32_t)(a_mn_major ? 1 : 0) << 15;
-  d |= (uint32_t)(b_mn_major ? 1 : 0) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
 
@@ -377,7 +228,7 @@ SDXE_DEVINL float gelu_erf_f(float x) { return 0.5f * x * (1.f + erff(x * 0.7071
 //   gelu(x) = x/2 (1 + erf z) = max(x, 0) - |x|/2 P(t) e^{-z^2}        (both signs of x)
 // and with u = x sqrt(log2(e) / 2) (so that e^{-z^2} = 2^{-u^2}) the constants |z| / |u| and |x| / (2 |u|) fold into p and
 // into P's coefficients: 11 FP32-pipe instructions + 2 MUFU per element (the textbook arrangement below took 15 + 2, and
-// the GEGLU epilogue is instruction-bound: profiles/r1_notes.md finding 3).
+// the GEGLU epilogue is instruction-bound).
 #ifndef SDXE_GELU_V1
 SDXE_DEVINL float gelu_fast_f(float x) {
   constexpr float C = 0.84932180028801904f;        // sqrt(log2(e) / 2)
@@ -439,7 +290,7 @@ int make_tmap_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int 
 int make_tmap_nhwc_s2(CUtensorMap* out, const void* base, int N, int H, int W, int C, int bw, int bh, int bn);
 
 int num_sms();
-bool pdl_enabled();  // SDXE_PDL=1 turns programmatic dependent launch on (default off: measured 1-2 % slower)
+bool pdl_enabled();  // SDXE_PDL=1 turns programmatic dependent launch on (default off)
 
 // Launch with the programmatic-stream-serialization attribute (see pdl_wait above). Only for kernels that call
 // pdl_wait() before touching global memory.

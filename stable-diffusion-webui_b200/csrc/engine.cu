@@ -318,9 +318,9 @@ struct Builder {
     }
     if (o.emit) {
       const int num_n = (a.N + a.BN - 1) / a.BN;
-      o.emit->buf = e->alloc((size_t)2 * num_n * M * sizeof(float2));
+      o.emit->buf = e->alloc((size_t)num_n * M * sizeof(float2));
       o.emit->p = (const float2*)o.emit->buf.p;
-      o.emit->parts = 2 * num_n;
+      o.emit->parts = num_n;
       a.stat_out = (float2*)o.emit->buf.p;
     }
     ECHK(gemm_finish_args(a, W.w, std::max(W.N, W.Nrows), W.ld));
@@ -435,20 +435,21 @@ struct Builder {
   int attention(const void* q, const void* k, const void* v, int B, int H, int Nq, int Nk, int d, int ldq, int ldkv,
                 float scale, void* out, int ldo, int dv_total) {
     const int dpad = (d + 63) / 64 * 64;
-    // dv_total > 256 (VAE, d = 512): passes over 256-wide slices of V
-    for (int v0 = 0; v0 < dv_total; v0 += 256) {
-      const int dv = std::min(256, dv_total - v0);
+    // value columns in passes of at most ATTN_MAX_DV (VAE d = 512, SD1.5 d = 160)
+    for (int v0 = 0; v0 < dv_total; v0 += ATTN_MAX_DV) {
+      const int dv = std::min(ATTN_MAX_DV, dv_total - v0);
       const int dvpad = (dv + 63) / 64 * 64;
       AttnArgs a;
       memset(&a, 0, sizeof(a));
-      ECHK(make_tmap_heads(&a.tmQ, q, d, Nq, H, B, ldq, d, (int64_t)Nq * ldq, 128));
-      ECHK(make_tmap_heads(&a.tmK, k, d, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, 128));
-      ECHK(make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, 128));
+      ECHK(make_tmap_heads(&a.tmQ, q, d, Nq, H, B, ldq, d, (int64_t)Nq * ldq, ATTN_Q_BOX_ROWS));
+      ECHK(make_tmap_heads(&a.tmK, k, d, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, ATTN_KV_BOX_ROWS));
+      ECHK(make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, ATTN_KV_BOX_ROWS));
       a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk;
       a.dqk_slabs = dpad / 64;
       a.dv_slabs = dvpad / 64;
-      a.dv = dv_total > 256 ? dv : d;
+      a.dv = dv;
       a.dqk = d;
+      a.out_hstride = dv_total;
       a.scale_log2 = scale * 1.4426950408889634f;
       a.out = out; a.ldo = ldo; a.out_col0 = v0;
       const bool b = bf16;

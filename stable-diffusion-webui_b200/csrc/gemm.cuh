@@ -1,4 +1,4 @@
-// Argument block of the tcgen05 GEMM / implicit-GEMM convolution kernel (gemm.cu).
+// Argument block of the wgmma GEMM / implicit-GEMM convolution kernel (gemm.cu).
 #pragma once
 #include "common.cuh"
 
@@ -13,18 +13,10 @@ struct alignas(64) GemmArgs {
   CUtensorMap tmA;   // 2D: [M, K1] 16-bit, box 64 x 128.  conv: NHWC [N,H,W,C], box 64 x bw x bh x bn
   CUtensorMap tmA2;  // optional second K segment (skip-concat read as two K-segments), 2D only
   CUtensorMap tmB;   // weights [N, K] K-contiguous, box 64 x BN
-  // epilogue: every output chunk (32 rows x 32 columns of one epilogue warp) leaves through a TMA store from a swizzled
-  // staging buffer, the residual chunk arrives the same way (whole 64-byte row pieces -> full-line L2 transactions
-  // instead of 32 scattered 16-byte accesses per warp instruction). The *16 maps serve a tile's 16-column tail chunk.
-  CUtensorMap tmO, tmO16;  // out [M, ldo]: box 32 x 32 (64B swizzle) / 16 x 32 (32B swizzle); rows >= M, cols >= N clipped
-  CUtensorMap tmR, tmR16;  // residual [M, ldr], same boxes (only when residual != null)
   int M, N, K;       // problem (conv: K = 9 * Cin, M = N_img * H * W)
   int K1;            // K elements sourced from tmA (== K when there is no second segment)
   int BN;            // tile width (multiple of 16, <= 256)
   int num_stages;
-  int epi_bufs;      // staging chunks per epilogue warp (set by gemm_finish_args): plain 1-2, residual 2-4
-  int res_dist;      // residual prefetch distance in chunks (set by gemm_finish_args): 1, or 2 with four buffers
-  unsigned long long* trace;  // SDXE_GEMM_TRACE builds: clock64 timeline of CTA 0 (see gemm.cu), else unused
   int conv;          // 0 = plain GEMM, 1 = 3x3 stride-1 pad-1 NHWC implicit GEMM, 2 = 3x3 stride-2 (tmA = make_tmap_nhwc_s2)
   int pad_lo;        // conv == 2: zero rows / columns before the image (1: ldm UNet Downsample, 0: VAE encoder pad (0,1,0,1))
   int cblocks;       // conv: Cin / 64
@@ -32,7 +24,6 @@ struct alignas(64) GemmArgs {
   int bh, bn;
   int epi;
   int ldrv;          // row pitch (elements) of rowvec
-  int cluster;       // 1, or 2: CTA pairs (consecutive m-tiles, same n-tile) share the B tile through TMA multicast
   const float* bias;    // [N] (EPI_GEGLU: interleaved like the weights) or null
   const float* rowvec;  // [M / rows_per_sample, N] per-sample vector added to every row of the sample, or null
   int rows_per_sample;
@@ -48,7 +39,7 @@ struct alignas(64) GemmArgs {
   int ln_parts;
   float ln_inv_c, ln_eps;   // 1 / K (the normalised width), epsilon
   // emit per-row partial statistics of the (rounded) output for a consumer's LayerNorm fold:
-  float2* stat_out;         // [2 * num_n][M]: part (n_blk * 2 + warp half); null = off. Needs EPI_PLAIN, no rowvec.
+  float2* stat_out;         // [num_n][M]: part n_blk; null = off. Needs EPI_PLAIN, no rowvec.
 };
 
 // Launch on `stream`. bf16 selects the 16-bit format of A/B/out/residual. Returns 0 / -1.
@@ -56,10 +47,9 @@ int gemm_launch(const GemmArgs& a, bool bf16, cudaStream_t stream);
 int gemm_init();  // one-time kernel attribute setup (call before any stream capture)
 // Tile-width heuristic: pick BN for an [M, N] output (geglu needs BN % 32 == 0 and N % BN == 0).
 int gemm_pick_bn(int M, int N, int K, int epi);
-int gemm_pick_stages(int BN, int epi_bufs);
-int gemm_pick_cluster(int M, int BN);  // 2 when CTA pairs (cta_group::2) are enabled and the geometry allows, else 1
-// After M/N/K/K1/BN/epi/tmA/out/ldo/residual/ldr are set: picks cluster + stage count, builds tmB over the packed
-// weights W [w_rows, K] (row pitch w_ld) and the epilogue's store / residual maps.
+int gemm_pick_stages(int BN);
+// After M/N/K/K1/BN/epi/tmA/out/ldo/residual/ldr are set: picks the stage count and builds tmB over the packed
+// weights W [w_rows, K] (row pitch w_ld).
 int gemm_finish_args(GemmArgs& a, const void* W, int64_t w_rows, int64_t w_ld);
 // 128-pixel tile of the implicit-GEMM conv as a TMA box (bw x bh x bn); false if (H, W) needs the im2col path.
 bool conv_tile_shape(int H, int W, int* bw, int* bh, int* bn);

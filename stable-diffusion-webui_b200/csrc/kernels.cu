@@ -163,7 +163,7 @@ __global__ void gn_apply_kernel(const uint4* __restrict__ x1, int c1, const uint
 // memory — one global read, fp32 two-pass statistics (mean, then centred second moment) from smem, one global write.
 // Replaces stats + finalize + apply (2 reads, 1 write, 3 launches) for the small tensors (strip hw * cpg * 2 B <= 48 KB:
 // the 8x8 / 16x16 and narrow 32x32 levels, where the three launches are latency-bound); larger tensors keep the
-// three-kernel streaming path (measured: 64x64x320 39 us vs 62 us one-pass).
+// three-kernel streaming path.
 // Thread -> (pixel lane, channel pair): the channel pair is fixed per thread, so gamma / beta / source pointer live in
 // registers and the loops carry no divisions. Fixed reduction order: bit-identical on replay.
 template <bool BF16, bool SILU>
@@ -265,7 +265,7 @@ int group_norm_launch(const void* x1, int c1, const void* x2, int c2, const floa
     if (onepass < 0) { const char* e = getenv("SDXE_GN_ONEPASS"); onepass = e ? atoi(e) : 1; }
     const int cpg = C / groups;
     const size_t strip = (size_t)hw * cpg * 2;
-    // measured crossover: one CTA per strip wins up to ~48 KB (enough CTAs per SM to hide its serial passes); the
+    // crossover: one CTA per strip wins up to ~48 KB (enough CTAs per SM to hide its serial passes); the
     // wide 64x64 / 32x32 tensors are faster through the three streaming kernels
     if (onepass && cpg % 2 == 0 && cpg / 2 <= 256 && strip <= 48 * 1024) {
       const int threads = strip >= 32 * 1024 ? 512 : 256;
@@ -610,12 +610,11 @@ int timestep_embedding_launch(const void* t, int t_dtype, float* out, int m, int
 
 // Skinny linear (a handful of rows against a wide weight matrix: time_embed, label_emb, all emb_layers in one launch):
 // out[M <= 16 per pass, N] = in[M, K] (fp32 holding 16-bit values) x W[N, K]^T. Sixteen rows are exactly one m16n8k16
-// warp-MMA tile — far below tcgen05's 64-row minimum, so this one op uses mma.sync: the kernel only has to stream the
+// warp-MMA tile — far below wgmma's 64-row minimum, so this one op uses mma.sync: the kernel only has to stream the
 // weight matrix once at HBM speed. A block stages its 16 input rows in shared memory as 16-bit (lossless: every producer
 // rounds to the model dtype); each warp owns 8 output features; per 32 k a lane reads ONE 16-byte weight vector (its
 // feature gid, k = 32 s + 8 tig .. + 7) and two 16-byte activation vectors (rows gid, gid + 8, same k) and issues two
 // MMAs — the k index inside a 32-block is permuted identically for both operands, which a dot product does not see.
-// (History: FMA versions of this op ran the 16 x 20480 x 1280 emb_layers product at 112 us and 66 us.)
 constexpr int SKL_WARPS = 8;
 template <bool BF16>
 SDXE_DEVINL void mma_16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
@@ -821,7 +820,7 @@ int ln_fold_launch(void* w, int rows, int K, int ld, const float* gamma, const f
 // =============================================================================================================
 // CLIP text encoder pieces (row N4: FrozenCLIPEmbedder / FrozenOpenCLIPEmbedder2 `transformer`,
 // modules/sd_hijack_clip.py:351-360, modules/sd_hijack_open_clip.py:29-71). 77-token sequences: launch-latency-sized
-// work, so plain CUDA-core kernels; the projections run on the tcgen05 GEMM with the LayerNorms folded in.
+// work, so plain CUDA-core kernels; the projections run on the wgmma GEMM with the LayerNorms folded in.
 // =============================================================================================================
 // x[m, :] = round16(tok[ids[m], :] + pos[m % T, :]); also the row's (sum, sum of squares) for the first folded LayerNorm.
 template <bool BF16>

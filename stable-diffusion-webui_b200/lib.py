@@ -98,7 +98,7 @@ def load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise SdxeError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). This engine has no CPU or PyTorch fallback."
+            "(nvcc, sm_90a). This engine has no CPU or PyTorch fallback."
         )
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():

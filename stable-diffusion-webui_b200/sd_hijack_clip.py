@@ -9,7 +9,7 @@ running on the sdxe engine. Host mirror of modules/sd_hijack_clip.py (same class
   emphasis options                                   modules/sd_emphasis.py:24-70 (None / Ignore / Original / No norm)
 
 `encode_with_transformers` = `sdxe_clip_forward` (engine kind SDXE_MODEL_CLIP_TEXT): embeddings, causal self-attention,
-quick-GELU MLP, LayerNorms folded into the tcgen05 GEMMs. The tokenizer (BPE vocabulary files) is injected by the caller —
+quick-GELU MLP, LayerNorms folded into the wgmma GEMMs. The tokenizer (BPE vocabulary files) is injected by the caller —
 any object with the Hugging Face tokenizer surface the reference uses (`__call__(texts, truncation=False,
 add_special_tokens=False)["input_ids"]`, `get_vocab()`, `bos_token_id`, `eos_token_id`). Textual-inversion embeddings
 ("custom words", :162-176, 219; modules/sd_hijack.py:340-366): every wrapper owns an `embedding_db`
@@ -329,7 +329,7 @@ class FrozenOpenCLIPEmbedder2WithCustomWords(TextConditionalModel):
         last = z if self.layer != "penultimate" else self.engine.forward(tokens, layer=n, final_norm=True, fixes=rows_fix)
         eot = tokens.to(last.device).argmax(dim=-1)                      # open_clip pools at the highest token id = <end_of_text>
         rows = last[torch.arange(last.shape[0], device=last.device), eot].contiguous()
-        pooled = ops.gemm(rows, self.text_projection_t)                  # tcgen05 GEMM, M = number of prompts
+        pooled = ops.gemm(rows, self.text_projection_t)                  # wgmma GEMM, M = number of prompts
         z.pooled = pooled  # the reference attaches the attribute to the hidden-state tensor (sd_hijack_open_clip.py:60-64)
         return z
 

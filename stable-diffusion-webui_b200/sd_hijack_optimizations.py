@@ -102,7 +102,7 @@ def sdxe_attnblock_forward(self, x):
 
 class SdOptimizationSdxe(_Base):
     name = "sdxe"
-    label = "B200 tcgen05 flash attention"
+    label = "H100 wgmma flash attention"
     cmd_opt = "opt_sdxe_attention"
     # below the stock CUDA choices (xformers 100, Doggettx 90, sdp-no-mem 80, sdp 70; :51-143): "Automatic" keeps the
     # reference's behaviour, the user opts in through Settings -> Cross attention optimization -> sdxe. (The UNet seam,
@@ -114,7 +114,8 @@ class SdOptimizationSdxe(_Base):
         self._saved = []
 
     def is_available(self):
-        return torch.cuda.is_available() and torch.cuda.get_device_capability()[0] == 10
+        # libsdxe.so holds sm_90a code only: it runs on Hopper (compute capability 9.0) and nothing else
+        return torch.cuda.is_available() and torch.cuda.get_device_capability() == (9, 0)
 
     def apply(self, classes=None):
         """classes: optional {"CrossAttention": [cls...], "AttnBlock": [cls...]}; default = ldm + sgm classes."""
