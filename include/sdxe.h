@@ -12,6 +12,9 @@
  *                          inside scaled_dot_product_attention_forward (:508-546) and sdp_attnblock_forward (:637-655)
  *   sdxe_vae_decode     <- modules/sd_samplers_common.py:58   model.decode_first_stage(z)  (AutoencoderKL.decode)
  *   sdxe_cfg_combine    <- modules/sd_samplers_cfg_denoiser.py:74-82   CFGDenoiser.combine_denoised
+ *   sdxe_cfg_combine_affine
+ *                       <- the same combine behind CFGDenoiserTimesteps (modules/sd_samplers_timesteps.py: raw eps,
+ *                          get_pred_x0, CFG++'s last_noise_uncond) and CFGDenoiserLCM (modules/sd_samplers_lcm.py:50-63)
  *   sdxe_denoiser_in / sdxe_denoiser_out
  *                       <- k_diffusion/external.py DiscreteEpsDDPMDenoiser.forward (c_in scaling, x + eps*c_out;
  *                          un-vendored dependency pinned at modules/launch_utils.py:357)
@@ -181,9 +184,20 @@ int sdxe_cfg_combine(const float* x, const void* eps, const float* sigma, float 
 int sdxe_cfg_combine_multi(const float* x, const void* eps, const float* sigma, const int32_t* row_ptr,
                            const int32_t* cond_rows, const float* cond_w, const int32_t* uncond_rows, float* denoised,
                            int B, int64_t elems, int eps_dtype, void* stream);
+/* Combine for denoisers whose per-row output is affine in (x[b], eps[r]) with per-image coefficients (DDIM / PLMS / UniPC:
+ * raw eps, cx = 0, ce = 1; LCM: c_out'(x - sigma eps) + c_skip' x). With the CSR rows of sdxe_cfg_combine_multi:
+ *   out[b] = cx[b] x[b] + ce[b] (e_u + sum_k cond_w[k] (e_k - e_u)),  e_u = eps[uncond_rows[b]].
+ * Optional, in the same pass (NULL to skip): x0_out[b] = x0_coef[2b] x[b] + x0_coef[2b+1] eps[cond_rows[row_ptr[b]]]
+ * (the timestep samplers' pred_x0 of the first cond, returned by an interrupted job) and uncond_out[b] = e_u as fp32
+ * (DDIM CFG++). cx, ce: fp32[B], x0_coef: fp32[2B] (device). eps is 16-bit or fp32. */
+int sdxe_cfg_combine_affine(const float* x, const void* eps, const int32_t* row_ptr, const int32_t* cond_rows,
+                            const float* cond_w, const int32_t* uncond_rows, const float* cx, const float* ce, float* out,
+                            const float* x0_coef, float* x0_out, float* uncond_out, int B, int64_t elems, int eps_dtype,
+                            void* stream);
 /* out = c0 p0 + c1 p1 + c2 p2 + c3 p3 over fp32 latents (p1..p3 may be NULL, out may alias an input): the step update of
  * the remaining k-diffusion samplers (Euler, Heun, DPM2, DPM2 a, DPM++ 2S a, LMS, Restart; selected at
- * modules/sd_samplers_kdiffusion.py:11-27) with the step's scalars computed on the host. */
+ * modules/sd_samplers_kdiffusion.py:11-27), of DDIM / DDIM CFG++ / PLMS / UniPC / LCM, with the step's scalars computed on
+ * the host. */
 int sdxe_lincomb(float* out, const float* p0, float c0, const float* p1, float c1, const float* p2, float c2, const float* p3,
                  float c3, int64_t total, void* stream);
 /* x <- x + (x - denoised)/sigma * (sigma_down - sigma) + noise * sigma_up  (noise may be NULL when sigma_up == 0). */

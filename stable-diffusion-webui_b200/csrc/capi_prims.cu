@@ -153,6 +153,18 @@ int sdxe_cfg_combine_multi(const float* x, const void* eps, const float* sigma, 
   return cfg_combine_multi_launch(x, eps, sigma, row_ptr, cond_rows, cond_w, uncond_rows, denoised, B, elems, eps_dtype,
                                   (cudaStream_t)stream);
 }
+int sdxe_cfg_combine_affine(const float* x, const void* eps, const int32_t* row_ptr, const int32_t* cond_rows,
+                            const float* cond_w, const int32_t* uncond_rows, const float* cx, const float* ce, float* out,
+                            const float* x0_coef, float* x0_out, float* uncond_out, int B, int64_t elems, int eps_dtype,
+                            void* stream) {
+  if (!x || !eps || !row_ptr || !cond_rows || !cond_w || !uncond_rows || !cx || !ce || !out || (x0_out && !x0_coef) ||
+      B < 0 || elems < 0 || (eps_dtype != SDXE_F32 && !is16(eps_dtype))) {
+    set_last_error(__FILE__, __LINE__, "sdxe_cfg_combine_affine: bad argument");
+    return -1;
+  }
+  return cfg_combine_affine_launch(x, eps, row_ptr, cond_rows, cond_w, uncond_rows, cx, ce, out, x0_coef, x0_out,
+                                   uncond_out, B, elems, eps_dtype, (cudaStream_t)stream);
+}
 int sdxe_euler_ancestral_step(float* x, const float* denoised, const float* noise, float sigma, float sigma_down,
                               float sigma_up, int64_t total, void* stream) {
   return euler_a_step_launch(x, denoised, noise, sigma, sigma_down, sigma_up, total, (cudaStream_t)stream);

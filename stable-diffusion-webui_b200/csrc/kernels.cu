@@ -1060,6 +1060,47 @@ int cfg_combine_multi_launch(const float* x, const void* eps, const float* sigma
   return 0;
 }
 
+// CFG combine for denoisers whose per-row output is affine in (x_b, eps_r) with coefficients shared by all rows of image b
+// (timestep denoisers: raw eps; LCM: c_out'(x - sigma eps) + c_skip' x). Then the guided output is also affine:
+//   out_b = cx[b] x_b + ce[b] (e_u + sum_k w_k (e_k - e_u)).
+// Optional side outputs, same pass: x0_out_b = x0_coef[2b] x_b + x0_coef[2b+1] e_{first cond row of b} (the timestep
+// path's pred_x0, the sampler's last_latent) and uncond_out_b = e_u as fp32 (CFG++ steps along the uncond noise).
+__global__ void cfg_combine_affine_kernel(const float* __restrict__ x, const void* __restrict__ eps,
+                                          const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ cond_rows,
+                                          const float* __restrict__ cond_w, const int32_t* __restrict__ uncond_rows,
+                                          const float* __restrict__ cx, const float* __restrict__ ce, float* __restrict__ out,
+                                          const float* __restrict__ x0_coef, float* __restrict__ x0_out,
+                                          float* __restrict__ uncond_out, int B, int64_t elems, int eps_dtype) {
+  const int64_t total = B * elems;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int b = (int)(idx / elems);
+    const int64_t e = idx - b * elems;
+    const float xv = x[idx];
+    const float eu = load_any(eps, eps_dtype, (int64_t)uncond_rows[b] * elems + e);
+    const int k0 = row_ptr[b], k1 = row_ptr[b + 1];
+    float acc = eu;
+    for (int k = k0; k < k1; ++k) acc += (load_any(eps, eps_dtype, (int64_t)cond_rows[k] * elems + e) - eu) * cond_w[k];
+    out[idx] = cx[b] * xv + ce[b] * acc;
+    if (x0_out) {
+      const float e0 = load_any(eps, eps_dtype, (int64_t)cond_rows[k0] * elems + e);
+      x0_out[idx] = x0_coef[2 * b] * xv + x0_coef[2 * b + 1] * e0;
+    }
+    if (uncond_out) uncond_out[idx] = eu;
+  }
+}
+
+int cfg_combine_affine_launch(const float* x, const void* eps, const int32_t* row_ptr, const int32_t* cond_rows,
+                              const float* cond_w, const int32_t* uncond_rows, const float* cx, const float* ce, float* out,
+                              const float* x0_coef, float* x0_out, float* uncond_out, int B, int64_t elems, int eps_dtype,
+                              cudaStream_t s) {
+  const int64_t total = B * elems;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 8);
+  cfg_combine_affine_kernel<<<blocks, 256, 0, s>>>(x, eps, row_ptr, cond_rows, cond_w, uncond_rows, cx, ce, out, x0_coef,
+                                                   x0_out, uncond_out, B, elems, eps_dtype);
+  SDXE_LAUNCH_CHECK();
+  return 0;
+}
+
 // out = c0 p0 + c1 p1 + c2 p2 + c3 p3 (null pointers skipped; out may alias any input): the update of every k-diffusion
 // sampler step is such a combination of x, denoised, a second denoised / derivative and noise, with host-side scalars.
 __global__ void lincomb_kernel(float* __restrict__ out, const float* p0, float c0, const float* p1, float c1, const float* p2,

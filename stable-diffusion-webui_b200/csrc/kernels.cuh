@@ -66,6 +66,10 @@ int cfg_combine_launch(const float* x, const void* eps, const float* sigma, floa
 int cfg_combine_multi_launch(const float* x, const void* eps, const float* sigma, const int32_t* row_ptr,
                              const int32_t* cond_rows, const float* cond_w, const int32_t* uncond_rows, float* denoised,
                              int B, int64_t elems, int eps_dtype, cudaStream_t s);
+int cfg_combine_affine_launch(const float* x, const void* eps, const int32_t* row_ptr, const int32_t* cond_rows,
+                              const float* cond_w, const int32_t* uncond_rows, const float* cx, const float* ce, float* out,
+                              const float* x0_coef, float* x0_out, float* uncond_out, int B, int64_t elems, int eps_dtype,
+                              cudaStream_t s);
 int euler_a_step_launch(float* x, const float* den, const float* noise, float sigma, float sigma_down, float sigma_up,
                         int64_t total, cudaStream_t s);
 int dpmpp_2m_step_launch(float* x, const float* den, const float* old, float ratio, float neg_expm1, float c0, float c1,

@@ -82,6 +82,7 @@ SYMBOLS = {
     "sdxe_denoiser_in": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "sdxe_cfg_combine": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "sdxe_cfg_combine_multi": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int, c_void_p]),
+    "sdxe_cfg_combine_affine": (c_int, [c_void_p] * 12 + [c_int, c_int64, c_int, c_void_p]),
     "sdxe_lincomb": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_float, c_void_p, c_float, c_void_p, c_float, c_int64, c_void_p]),
     "sdxe_euler_ancestral_step": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_int64, c_void_p]),
     "sdxe_dpmpp_2m_step": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_int64, c_void_p]),

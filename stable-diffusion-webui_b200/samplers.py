@@ -9,11 +9,17 @@ and error behaviour, so parity tests read like the reference's own:
   sample_dpmpp_2m              k_diffusion/sampling.py (un-vendored; selected at sd_samplers_kdiffusion.py:11-27)
   setup_img2img_steps          modules/sd_samplers_common.py:22-31
   InterruptedException         modules/sd_samplers_common.py (raised when state.interrupted, cfg_denoiser.py:157-158)
+  Sampler                      modules/sd_samplers_common.py:229-332 (initialize / launch_sampling / callback_state)
+  create_sampler,
+  find_sampler_config          modules/sd_samplers.py:11-33 — one table of the k-diffusion samplers below, the timestep
+                               samplers (sd_samplers_timesteps.py: DDIM, DDIM CFG++, PLMS, UniPC) and LCM (sd_samplers_lcm.py)
 
 What is new: the UNet behind `inner_model` is the sdxe engine, and the per-step latent-space elementwise work
 (2B batch build + c_in, x + eps*c_out + CFG combine, sampler update) runs as three fused CUDA kernels from
 libsdxe.so instead of ~15 small PyTorch launches (SURVEY K9). The sigma schedule stays on the host
-(modules/sd_samplers_kdiffusion.py:127,132).
+(modules/sd_samplers_kdiffusion.py:127,132). CFGDenoiser keeps the three denoiser-specific steps in overridable methods
+(model_inputs: c_in and the UNet timestep; combine; last_latent) so that the timestep and LCM denoisers add only their
+differences; their combine is sdxe_cfg_combine_affine.
 """
 from __future__ import annotations
 
@@ -275,12 +281,74 @@ class CFGDenoiser:
             self._ctx_refs = (cond, uncond)  # the ids stay unique while the denoiser holds the objects
         return key
 
+    def model_inputs(self, sigma_in):
+        """Per UNet row: the input scaling c_in and the timestep the UNet sees (CompVisDenoiser.forward)."""
+        _, c_in = self.inner_model.get_scalings(sigma_in)
+        return c_in, self.inner_model.sigma_to_t(sigma_in)
+
+    def _csr(self, x, conds_list, skip_uncond, scale):
+        """Device tables of the general combine: row_ptr [B+1], cond_rows, cond_w (weight * scale), uncond_rows [B]."""
+        repeats = [len(c) for c in conds_list]
+        n_cond, batch_size = sum(repeats), len(conds_list)
+        wkey = ("csr", tuple(repeats), skip_uncond, tuple(w for c in conds_list for _, w in c), scale)
+
+        def build():
+            ptr, k = [0], 0
+            for n in repeats:
+                k += n
+                ptr.append(k)
+            # skipped uncond: the reference puts each image's FIRST cond result where the uncond result would be
+            urows = [c[0][0] for c in conds_list] if skip_uncond else [n_cond + i for i in range(batch_size)]
+            return (torch.tensor(ptr, device=x.device, dtype=torch.int32),
+                    torch.tensor([j for c in conds_list for j, _ in c], device=x.device, dtype=torch.int32),
+                    torch.tensor([w * scale for c in conds_list for _, w in c], device=x.device, dtype=torch.float32),
+                    torch.tensor(urows, device=x.device, dtype=torch.int32))
+
+        return self._dev(wkey, build)
+
+    def combine(self, x, eps, sigma, sigma_in, conds_list, skip_uncond, scale):
+        """x_out = x_in + eps * c_out and the CFG combine, fused (:272-289). `scale`: cond_scale * cond_scale_miltiplier."""
+        lib = L.load()
+        stream = L.current_stream()
+        batch_size, elems = len(conds_list), x[0].numel()
+        n_cond = sum(len(c) for c in conds_list)
+        if self.need_last_noise_uncond and not skip_uncond:
+            c_out, _ = self.inner_model.get_scalings(sigma_in)
+            self.last_noise_uncond = x + eps[n_cond:].float() * c_out[n_cond:].view(-1, 1, 1, 1)
+        if skip_uncond:
+            scale = 1.0
+        denoised = torch.empty_like(x)
+        if n_cond == batch_size and not skip_uncond and all(c[0][1] == 1.0 for c in conds_list):
+            L.check(lib.sdxe_cfg_combine(L.ptr(x), L.ptr(eps), L.ptr(sigma), scale, L.ptr(denoised), batch_size, elems,
+                                         L.torch_dtype_code(eps.dtype), stream), "sdxe_cfg_combine")
+        else:
+            row_ptr, cond_rows, cond_w, uncond_rows = self._csr(x, conds_list, skip_uncond, scale)
+            L.check(lib.sdxe_cfg_combine_multi(L.ptr(x), L.ptr(eps), L.ptr(sigma), L.ptr(row_ptr), L.ptr(cond_rows), L.ptr(cond_w),
+                                               L.ptr(uncond_rows), L.ptr(denoised), batch_size, elems,
+                                               L.torch_dtype_code(eps.dtype), stream), "sdxe_cfg_combine_multi")
+        return denoised
+
+    def combine_affine(self, x, eps, conds_list, skip_uncond, scale, cx, ce, x0_coef=None, want_uncond=False):
+        """The CFG combine of a denoiser whose output per row is cx[b] * x[b] + ce[b] * eps[r] (sdxe_cfg_combine_affine).
+        Returns (out, pred_x0 of each image's first cond or None, uncond eps as fp32 or None)."""
+        row_ptr, cond_rows, cond_w, uncond_rows = self._csr(x, conds_list, skip_uncond, 1.0 if skip_uncond else scale)
+        out = torch.empty_like(x)
+        x0 = torch.empty_like(x) if x0_coef is not None else None
+        unc = torch.empty_like(x) if want_uncond else None
+        L.check(L.load().sdxe_cfg_combine_affine(L.ptr(x), L.ptr(eps), L.ptr(row_ptr), L.ptr(cond_rows), L.ptr(cond_w), L.ptr(uncond_rows),
+                                                 L.ptr(cx), L.ptr(ce), L.ptr(out), L.ptr(x0_coef), L.ptr(x0), L.ptr(unc), len(conds_list),
+                                                 x[0].numel(), L.torch_dtype_code(eps.dtype), L.current_stream()), "sdxe_cfg_combine_affine")
+        return out, x0, unc
+
+    def last_latent(self, denoised):
+        """What an interrupted job returns (the sampler's last_latent)."""
+        return denoised
+
     def forward(self, x, sigma, uncond, cond, cond_scale, s_min_uncond, image_cond):
         if state.interrupted or state.skipped:
             raise InterruptedException
         from . import prompt_parser
 
-        model = self.inner_model
         sd = self.sampler.sd_model
         lib = L.load()
         opts = self.opts
@@ -326,8 +394,7 @@ class CFGDenoiser:
             tensor, uncond = self.pad_cond_uncond(tensor, uncond)
         # ---- fused: x_in[r] = x[src[r]] * c_in[r] in the UNet's dtype (:203 + CompVisDenoiser c_in + the dtype cast of
         #      sd_hijack_unet.py:43-50)
-        c_out, c_in = model.get_scalings(sigma_in)
-        t = model.sigma_to_t(sigma_in)
+        c_in, t = self.model_inputs(sigma_in)
         elems = x[0].numel()
         x_in = torch.empty((rows,) + tuple(x.shape[1:]), dtype=sd.dtype_unet, device=x.device)
         stream = L.current_stream()
@@ -353,36 +420,10 @@ class CFGDenoiser:
             eps[n_cond:] = self._run_unet(x_in[n_cond:], t[n_cond:], uncond)
         for cb in self.on_cfg_denoised:
             cb(eps)
-        if self.need_last_noise_uncond and not skip_uncond:
-            self.last_noise_uncond = x + eps[n_cond:].float() * c_out[n_cond:].view(-1, 1, 1, 1)
-        # ---- x_out = x_in + eps * c_out and the CFG combine, fused (:272-289)
-        scale = 1.0 if skip_uncond else float(cond_scale) * self.cond_scale_miltiplier
-        denoised = torch.empty_like(x)
-        if plain and not skip_uncond and all(c[0][1] == 1.0 for c in conds_list):
-            L.check(lib.sdxe_cfg_combine(L.ptr(x), L.ptr(eps), L.ptr(sigma), scale, L.ptr(denoised), batch_size, elems,
-                                         L.torch_dtype_code(eps.dtype), stream), "sdxe_cfg_combine")
-        else:
-            wkey = ("csr",) + key + (tuple(w for c in conds_list for _, w in c), scale)
-
-            def build():
-                ptr, k = [0], 0
-                for n in repeats:
-                    k += n
-                    ptr.append(k)
-                # skipped uncond: the reference puts each image's FIRST cond result where the uncond result would be
-                urows = [c[0][0] for c in conds_list] if skip_uncond else [n_cond + i for i in range(batch_size)]
-                return (torch.tensor(ptr, device=x.device, dtype=torch.int32),
-                        torch.tensor([j for c in conds_list for j, _ in c], device=x.device, dtype=torch.int32),
-                        torch.tensor([w * scale for c in conds_list for _, w in c], device=x.device, dtype=torch.float32),
-                        torch.tensor(urows, device=x.device, dtype=torch.int32))
-
-            row_ptr, cond_rows, cond_w, uncond_rows = self._dev(wkey, build)
-            L.check(lib.sdxe_cfg_combine_multi(L.ptr(x), L.ptr(eps), L.ptr(sigma), L.ptr(row_ptr), L.ptr(cond_rows), L.ptr(cond_w),
-                                               L.ptr(uncond_rows), L.ptr(denoised), batch_size, elems,
-                                               L.torch_dtype_code(eps.dtype), stream), "sdxe_cfg_combine_multi")
+        denoised = self.combine(x, eps, sigma, sigma_in, conds_list, skip_uncond, float(cond_scale) * self.cond_scale_miltiplier)
         if not self.mask_before_denoising and self.mask is not None:
             denoised = self._apply_blend(denoised)
-        self.sampler.last_latent = denoised
+        self.sampler.last_latent = self.last_latent(denoised)
         for cb in self.on_cfg_after_cfg:
             r = cb(denoised)
             if r is not None:
@@ -747,12 +788,61 @@ class SchedulerOptions:
     sgm_noise_multiplier = False
 
 
-class KDiffusionSampler:
+class Sampler:
+    """What every sampler shares (modules/sd_samplers_common.py:229-332 Sampler): per-job initialisation, the
+    interrupt-to-last_latent rule and the step callback."""
+
+    eta_default = 1.0  # opts.eta_ancestral; the timestep samplers use opts.eta_ddim
+
+    def initialize(self, p) -> dict:
+        """modules/sd_samplers_common.py:288-333: per-job state + the sampler function's optional arguments."""
+        import inspect
+
+        self.p = p
+        cfg = self.model_wrap_cfg
+        cfg.p = p
+        cfg.mask = getattr(p, "mask", None)
+        cfg.nmask = getattr(p, "nmask", None)
+        cfg.step = 0
+        self.eta = p.eta if getattr(p, "eta", None) is not None else self.eta_default
+        self.s_min_uncond = getattr(p, "s_min_uncond", 0.0)
+        params = inspect.signature(self.func).parameters
+        kw = {}
+        for name in sampler_extra_params.get(self.func, []):
+            if hasattr(p, name) and name in params:
+                kw[name] = getattr(p, name)
+        if "s_tmax" in kw and not kw["s_tmax"]:
+            kw["s_tmax"] = float("inf")  # 0 = inf
+        if "eta" in params:
+            kw["eta"] = self.eta
+        if "noise_sampler" in params:
+            kw["noise_sampler"] = lambda sigma, sigma_next: p.rng.next()  # TorchHijack.randn_like -> p.rng.next()
+        return kw
+
+    def launch_sampling(self, steps, func):
+        self.model_wrap_cfg.steps = steps
+        self.model_wrap_cfg.total_steps = steps
+        state.sampling_steps = steps
+        state.sampling_step = 0
+        try:
+            return func()
+        except InterruptedException:
+            return self.last_latent
+
+    def callback_state(self, d):
+        state.sampling_step = d["i"]
+
+
+class KDiffusionSampler(Sampler):
     def __init__(self, funcname_or_label, sd_model, options=None):
-        key = funcname_or_label.lower() if isinstance(funcname_or_label, str) else None
-        if key not in _sampler_map:
-            raise L.SdxeError(f"sampler {funcname_or_label!r} is not mirrored (available: " + ", ".join(x[0] for x in samplers_k_diffusion) + ")")
-        self.label, self.func, self.options = _sampler_map[key]
+        """funcname_or_label: a label or alias of the k-diffusion table, or a sampler function (options then start empty)."""
+        if callable(funcname_or_label):
+            self.label, self.func, self.options = funcname_or_label.__name__, funcname_or_label, {}
+        else:
+            key = funcname_or_label.lower() if isinstance(funcname_or_label, str) else None
+            if key not in _sampler_map:
+                raise L.SdxeError(f"sampler {funcname_or_label!r} is not mirrored (available: " + ", ".join(x[0] for x in samplers_k_diffusion) + ")")
+            self.label, self.func, self.options = _sampler_map[key]
         if options:
             self.options = {**self.options, **options}
         self.sd_model = sd_model
@@ -805,44 +895,6 @@ class KDiffusionSampler:
             sigmas = torch.cat([sigmas[:-2], sigmas[-1:]])
         return sigmas.cpu()
 
-    def initialize(self, p) -> dict:
-        """modules/sd_samplers_common.py:288-333: per-job state + the sampler function's optional arguments."""
-        import inspect
-
-        self.p = p
-        cfg = self.model_wrap_cfg
-        cfg.p = p
-        cfg.mask = getattr(p, "mask", None)
-        cfg.nmask = getattr(p, "nmask", None)
-        cfg.step = 0
-        self.eta = p.eta if getattr(p, "eta", None) is not None else 1.0  # opts.eta_ancestral default
-        self.s_min_uncond = getattr(p, "s_min_uncond", 0.0)
-        params = inspect.signature(self.func).parameters
-        kw = {}
-        for name in sampler_extra_params.get(self.func, []):
-            if hasattr(p, name) and name in params:
-                kw[name] = getattr(p, name)
-        if "s_tmax" in kw and not kw["s_tmax"]:
-            kw["s_tmax"] = float("inf")  # 0 = inf
-        if "eta" in params:
-            kw["eta"] = self.eta
-        if "noise_sampler" in params:
-            kw["noise_sampler"] = lambda sigma, sigma_next: p.rng.next()  # TorchHijack.randn_like -> p.rng.next()
-        return kw
-
-    def launch_sampling(self, steps, func):
-        self.model_wrap_cfg.steps = steps
-        self.model_wrap_cfg.total_steps = steps
-        state.sampling_steps = steps
-        state.sampling_step = 0
-        try:
-            return func()
-        except InterruptedException:
-            return self.last_latent
-
-    def callback_state(self, d):
-        state.sampling_step = d["i"]
-
     def sample(self, p, x, conditioning, unconditional_conditioning, steps=None, image_conditioning=None):
         steps = steps or p.steps
         sigmas = self.get_sigmas(p, steps)
@@ -872,11 +924,36 @@ class KDiffusionSampler:
                                                                  sigmas=sigma_sched, **extra))
 
 
+def _all_samplers():
+    """label / alias (lower case) -> (label, function, options, constructor) over the k-diffusion, timestep and LCM tables
+    (modules/sd_samplers.py:11-16)."""
+    global _all_sampler_map
+    if _all_sampler_map is None:
+        from . import sd_samplers_lcm, sd_samplers_timesteps
+
+        table = {}
+        for rows, ctor in ((samplers_k_diffusion, KDiffusionSampler), (sd_samplers_timesteps.samplers_timesteps, sd_samplers_timesteps.CompVisSampler),
+                           (sd_samplers_lcm.samplers_lcm, sd_samplers_lcm.LCMSampler)):
+            for label, fn, aliases, opts in rows:
+                for name in [label] + aliases:
+                    table[name.lower()] = (label, fn, opts, ctor)
+        table["dpm++ 2m karras"] = table["dpm++ 2m"]  # pre-1.9 name (infotext compatibility)
+        _all_sampler_map = table
+    return _all_sampler_map
+
+
+_all_sampler_map = None
+
+
 def find_sampler_config(name):
     """modules/sd_samplers.py:18-24 — (label, function, options) of a sampler by label or alias, None when unknown."""
-    return _sampler_map.get(str(name).lower())
+    entry = _all_samplers().get(str(name).lower())
+    return None if entry is None else entry[:3]
 
 
-def create_sampler(name, model) -> KDiffusionSampler:
+def create_sampler(name, model) -> Sampler:
     """modules/sd_samplers.py:33."""
-    return KDiffusionSampler(name, model)
+    entry = _all_samplers().get(str(name).lower())
+    if entry is None:
+        raise L.SdxeError(f"sampler {name!r} is not mirrored (available: " + ", ".join(sorted({e[0] for e in _all_samplers().values()})) + ")")
+    return entry[3](entry[0], model)
