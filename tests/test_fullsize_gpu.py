@@ -184,19 +184,21 @@ def test_c4_sd15_hires_512_to_1024(cuda):
     _txt2img_case(cuda, "sd15", sp, 2, [torch.float16], 768, 0, 0.18215)
 
 
-@pytest.mark.parametrize("config,n,hw", [("sd15", 16, 64), ("sdxl", 8, 128)])
-def test_unet_forward_bench_shape(cuda, config, n, hw):
-    """One UNet forward at the CFG batch the bench runs: SD1.5 2B = 16 @ 64x64, SDXL 2B = 8 @ 128x128; fp16 and bf16."""
+@pytest.mark.parametrize("config,n,h,w", [("sd15", 16, 64, 64), ("sdxl", 8, 128, 128), ("sdxl", 4, 104, 152), ("sd15", 8, 64, 96)])
+def test_unet_forward_bench_shape(cuda, config, n, h, w):
+    """One UNet forward at the CFG batch the bench runs: SD1.5 2B = 16 @ 64x64, SDXL 2B = 8 @ 128x128; and at sizes
+    whose convolutions all go through im2col: SDXL's 1216x832 bucket (latent 104x152, ragged GEMM tiles, self-attention
+    over 3952 and 988 tokens) and SD1.5 at 768x512 (latent 64x96). fp16 and bf16."""
     spec, unet, vae, usd, vsd = _oracle_models(cuda, config, 3, 4)
     from sdwebui_b200.engine import UNetEngine
 
     del vae, vsd
     g = torch.Generator(device="cuda").manual_seed(9)
-    x = torch.randn(n, 4, hw, hw, device=cuda, generator=g)
+    x = torch.randn(n, 4, h, w, device=cuda, generator=g)
     t = torch.linspace(950.0, 20.5, n, device=cuda)
     ctx = torch.randn(n, 77, spec.context_dim, device=cuda, generator=g)
     y = torch.randn(n, spec.adm_in_channels, device=cuda, generator=g) if spec.adm_in_channels else None
-    print(f"\n{config} UNet forward n={n} @ {hw}x{hw}:")
+    print(f"\n{config} UNet forward n={n} @ {h}x{w}:")
     refs, ref32 = {}, {}
     for dt in (torch.float16, torch.bfloat16):
         xq, tq, cq, yq = x.to(dt), t.to(dt), ctx.to(dt), (y.to(dt) if y is not None else None)
@@ -225,26 +227,24 @@ def test_unet_forward_bench_shape(cuda, config, n, hw):
         _free()
 
 
-def test_vae_decode_1024(cuda):
-    """KL-f8 decoder at 128x128 latent -> 1024x1024, B=2: mid-block attention over 16384 tokens at d = 512, convs with
-    up to 2M output rows per image."""
+def _vae_decode_case(cuda, n, h, w, seed_w, seed_z):
     from oracle.vae import AutoencoderKLDecode, VAEConfig
     from sdwebui_b200 import checkpoint as C
     from sdwebui_b200.engine import VAEDecoderEngine, VAESpec
 
-    vsd = C.synthetic_state_dict(C.vae_decoder_param_shapes(VAESpec()), seed=8, device=cuda, dtype=torch.float32)
+    vsd = C.synthetic_state_dict(C.vae_decoder_param_shapes(VAESpec()), seed=seed_w, device=cuda, dtype=torch.float32)
     with torch.device(cuda):
         vae = AutoencoderKLDecode(VAEConfig()).eval()
     vae.load_state_dict(vsd)
-    g = torch.Generator(device="cuda").manual_seed(5)
-    z = torch.randn(2, 4, 128, 128, device=cuda, generator=g)
-    print("\nVAE decode 2 x 128x128 -> 1024x1024:")
+    g = torch.Generator(device="cuda").manual_seed(seed_z)
+    z = torch.randn(n, 4, h, w, device=cuda, generator=g)
+    print(f"\nVAE decode {n} x {h}x{w} -> {8 * h}x{8 * w}:")
     for dt in (torch.float16, torch.bfloat16):
         zq = z.to(dt)
         with torch.no_grad():
-            ref32 = torch.cat([vae.decode(zq[i:i + 1].float()) for i in range(2)])
+            ref32 = torch.cat([vae.decode(zq[i:i + 1].float()) for i in range(n)])
             v16 = copy.deepcopy(vae).to(dt)
-            ref16 = torch.cat([v16.decode(zq[i:i + 1]) for i in range(2)])
+            ref16 = torch.cat([v16.decode(zq[i:i + 1]) for i in range(n)])
         del v16
         eng = VAEDecoderEngine(VAESpec(), dtype=dt, device=cuda)
         eng.load_state_dict(vsd)
@@ -256,3 +256,15 @@ def test_vae_decode_1024(cuda):
         eng.close()
         del eng, ref32, ref16
         _free()
+
+
+def test_vae_decode_1024(cuda):
+    """KL-f8 decoder at 128x128 latent -> 1024x1024, B=2: mid-block attention over 16384 tokens at d = 512, convs with
+    up to 2M output rows per image."""
+    _vae_decode_case(cuda, 2, 128, 128, 8, 5)
+
+
+def test_vae_decode_832x1216(cuda):
+    """KL-f8 decoder at SDXL's 1216x832 bucket (latent 104x152), B=1: every conv through im2col, mid-block attention
+    over 15808 tokens (a ragged last KV block) at d = 512."""
+    _vae_decode_case(cuda, 1, 104, 152, 8, 6)

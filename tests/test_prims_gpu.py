@@ -71,7 +71,10 @@ def test_gemm_geglu(cuda, dtype, M, C):
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("n,h,w,cin,cout", [(2, 8, 8, 64, 64), (1, 16, 16, 128, 320), (2, 32, 32, 64, 128), (3, 64, 64, 64, 32),
                                             (1, 128, 128, 64, 64), (2, 16, 8, 64, 64), (16, 8, 8, 1280, 1280), (1, 64, 64, 320, 320),
-                                            (3, 8, 8, 128, 64)])
+                                            (3, 8, 8, 128, 64),
+                                            # tileable but not square: a partial last tile of several images, rows of 8
+                                            # or 16 pixels, a W of two 128-pixel boxes
+                                            (5, 8, 8, 64, 64), (2, 48, 16, 64, 128), (2, 24, 16, 320, 320), (1, 4, 256, 64, 64)])
 def test_conv3x3(cuda, dtype, n, h, w, cin, cout):
     from sdwebui_b200 import ops
 
@@ -93,6 +96,9 @@ def test_conv3x3(cuda, dtype, n, h, w, cin, cout):
     # short-KV persistent kernel (Nk <= 128, D <= 64): more items than SMs, ragged Nq, every key-count class
     (2, 8, 4096, 77, 40), (2, 10, 1024, 77, 64), (1, 3, 200, 77, 40), (1, 2, 128, 128, 64), (1, 2, 384, 100, 48),
     (1, 1, 64, 16, 8), (3, 5, 130, 1, 32), (16, 8, 4096, 77, 40),
+    # ragged last KV blocks: SDXL's UNet at 1216x832 (3952 and 988 tokens), SD1.5's first level at 768x512 (6144), and
+    # the VAE mid-block at 1216x832 (15808 tokens, d = 512 in four value passes)
+    (2, 10, 3952, 3952, 64), (2, 20, 988, 988, 64), (2, 10, 3952, 77, 64), (2, 8, 6144, 6144, 40), (1, 1, 15808, 15808, 512),
 ])
 def test_attention(cuda, dtype, B, H, Nq, Nk, D):
     from sdwebui_b200 import ops
@@ -109,14 +115,17 @@ def test_attention(cuda, dtype, B, H, Nq, Nk, D):
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("n,hw,c,silu", [(2, 64, 64, True), (3, 4096, 320, True), (2, 1024, 960, False), (1, 256, 2560, True),
-                                         (1, 65536, 128, True)])
-def test_group_norm(cuda, dtype, n, hw, c, silu):
+@pytest.mark.parametrize("n,h,w,c,silu", [(2, 8, 8, 64, True), (3, 64, 64, 320, True), (2, 32, 32, 960, False), (1, 16, 16, 2560, True),
+                                           (1, 256, 256, 128, True),
+                                           # UNet levels of a 1216x832 image: streaming (hw * C/32 * 2 B > 48 KB) and
+                                           # one-pass (the last, SD1.5's 13x19 level)
+                                           (2, 104, 152, 320, True), (2, 52, 76, 640, False), (2, 26, 38, 1280, True),
+                                           (4, 13, 19, 1280, False)])
+def test_group_norm(cuda, dtype, n, h, w, c, silu):
     from sdwebui_b200 import ops
 
     g = torch.Generator(device="cuda").manual_seed(c)
-    h = int(math.isqrt(hw))
-    x = (torch.randn(n, h, hw // h, c, device=cuda, generator=g) * 2 + 0.5).to(dtype)
+    x = (torch.randn(n, h, w, c, device=cuda, generator=g) * 2 + 0.5).to(dtype)
     gamma = torch.randn(c, device=cuda, generator=g)
     beta = torch.randn(c, device=cuda, generator=g)
     out = ops.group_norm_nhwc(x, gamma, beta, 32, 1e-5, silu)
