@@ -15,9 +15,8 @@
  *   sdxe_cfg_combine_affine
  *                       <- the same combine behind CFGDenoiserTimesteps (modules/sd_samplers_timesteps.py: raw eps,
  *                          get_pred_x0, CFG++'s last_noise_uncond) and CFGDenoiserLCM (modules/sd_samplers_lcm.py:50-63)
- *   sdxe_denoiser_in / sdxe_denoiser_out
- *                       <- k_diffusion/external.py DiscreteEpsDDPMDenoiser.forward (c_in scaling, x + eps*c_out;
- *                          un-vendored dependency pinned at modules/launch_utils.py:357)
+ *   sdxe_denoiser_in    <- k_diffusion/external.py DiscreteEpsDDPMDenoiser.forward (c_in scaling; its x + eps*c_out runs
+ *                          inside sdxe_cfg_combine; un-vendored dependency pinned at modules/launch_utils.py:357)
  *   sdxe_euler_ancestral_step / sdxe_dpmpp_2m_step
  *                       <- k_diffusion/sampling.py sample_euler_ancestral / sample_dpmpp_2m loop bodies
  *                          (called through modules/sd_samplers_kdiffusion.py:230)

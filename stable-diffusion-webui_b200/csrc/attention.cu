@@ -18,6 +18,7 @@
 #include "attention.cuh"
 #include "wgmma.cuh"
 #include <algorithm>
+#include <cstring>
 
 namespace sdxe {
 
@@ -31,7 +32,6 @@ static constexpr int SMEM_BUDGET = 227 * 1024;
 template <bool BF16, int NVS>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_constant__ AttnArgs a) {
   using T = T16<BF16>;
-  pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
@@ -58,7 +58,6 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
     tma_prefetch_desc(&a.tmV);
   }
   __syncthreads();
-  pdl_wait();  // q / k / v of the producing GEMM are complete; the output buffer is free
 
   if (warp == CONSUMER_WARPS) {
     // ---------------------------------------------------------------- producer (converged warp, elected issue)
@@ -240,7 +239,34 @@ int attention_launch(const AttnArgs& a_in, bool bf16, cudaStream_t stream) {
   const size_t smem = fixed + (size_t)a.num_slots * (SLAB_BYTES + 16);
   if (attention_init() != 0) return -1;
   dim3 grid((a.Nq + 127) / 128, a.B * a.H);
-  SDXE_CUDA_CHECK(launch_k(attention_variant(bf16, a.dv_slabs), grid, dim3(ATT_THREADS), smem, stream, a));
+  const AttnKernel kern = attention_variant(bf16, a.dv_slabs);
+  kern<<<grid, ATT_THREADS, smem, stream>>>(a);
+  SDXE_LAUNCH_CHECK();
+  return 0;
+}
+
+int attention_args(std::vector<AttnArgs>& passes, const AttnView& q, const AttnView& k, const AttnView& v, int B, int H,
+                   int Nq, int Nk, int dqk, int dv, float scale, void* out, int ldo, int out_hstride) {
+  passes.clear();
+  for (int v0 = 0; v0 < dv; v0 += ATTN_MAX_DV) {  // the O accumulator of a pass lives in registers
+    const int w = std::min(ATTN_MAX_DV, dv - v0);
+    AttnArgs a;
+    memset(&a, 0, sizeof(a));
+    // a 64-wide box reaching past the head dim (or the pass's value columns) is zero-filled by TMA
+    if (make_tmap_heads(&a.tmQ, q.p, dqk, Nq, H, B, q.tok_stride, q.head_stride, q.batch_stride, ATTN_Q_BOX_ROWS)) return -1;
+    if (make_tmap_heads(&a.tmK, k.p, dqk, Nk, H, B, k.tok_stride, k.head_stride, k.batch_stride, ATTN_KV_BOX_ROWS)) return -1;
+    if (make_tmap_heads(&a.tmV, (const uint16_t*)v.p + v0, w, Nk, H, B, v.tok_stride, v.head_stride, v.batch_stride,
+                        ATTN_KV_BOX_ROWS))
+      return -1;
+    a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk;
+    a.dqk_slabs = (dqk + 63) / 64;
+    a.dv_slabs = (w + 63) / 64;
+    a.dv = w;
+    a.dqk = dqk;
+    a.scale_log2 = scale * 1.4426950408889634f;
+    a.out = out; a.ldo = ldo; a.out_col0 = v0; a.out_hstride = out_hstride;
+    passes.push_back(a);
+  }
   return 0;
 }
 

@@ -1,6 +1,7 @@
 // Argument block of the wgmma flash-attention kernel (attention.cu).
 #pragma once
 #include "common.cuh"
+#include <vector>
 
 namespace sdxe {
 
@@ -27,6 +28,16 @@ static constexpr int ATTN_Q_BOX_ROWS = 128;
 static constexpr int ATTN_KV_BOX_ROWS = 64;
 static constexpr int ATTN_MAX_DV = 128;  // value columns per pass
 
+// One operand of attention as a per-head view: element j of token t, head h, batch b at
+// p + b * batch_stride + t * tok_stride + h * head_stride + j (strides in elements, multiples of 8).
+struct AttnView {
+  const void* p;
+  int64_t tok_stride, head_stride, batch_stride;
+};
+// softmax(q k^T * scale) v with q / k of head dim dqk and dv value columns per head, written to out[b * Nq + t, h * out_hstride
+// + j] (row pitch ldo). Value columns run in passes of at most ATTN_MAX_DV: one AttnArgs per pass. Returns 0 / -1.
+int attention_args(std::vector<AttnArgs>& passes, const AttnView& q, const AttnView& k, const AttnView& v, int B, int H,
+                   int Nq, int Nk, int dqk, int dv, float scale, void* out, int ldo, int out_hstride);
 int attention_launch(const AttnArgs& a, bool bf16, cudaStream_t stream);
 int attention_init();
 

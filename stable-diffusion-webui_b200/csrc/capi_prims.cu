@@ -6,6 +6,7 @@
 #include "kernels.cuh"
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 using namespace sdxe;
 
@@ -21,33 +22,15 @@ int sdxe_attention(const void* q, const void* k, const void* v, void* out, int B
                    float scale, int dtype, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!is16(dtype) || D % 8 != 0 || D > 512 || D <= 0) { set_last_error(__FILE__, __LINE__, "sdxe_attention: dtype/D"); return -2; }
-  const bool bf16 = dtype == SDXE_BF16;
-  const int Dpad = (D + 63) / 64 * 64;
-  // value dim is processed in passes of at most ATTN_MAX_DV columns (the O accumulator lives in registers)
-  int rc = 0;
-  for (int v0 = 0; v0 < D && rc == 0; v0 += ATTN_MAX_DV) {
-    const int dv = std::min(ATTN_MAX_DV, D - v0);
-    AttnArgs a;
-    memset(&a, 0, sizeof(a));
-    // [B, H, N, D] contiguous seen as (d, token, head, batch); boxes reaching past D are zero-filled by TMA
-    if (make_tmap_heads(&a.tmQ, q, D, Nq, H, B, D, (int64_t)Nq * D, (int64_t)H * Nq * D, ATTN_Q_BOX_ROWS)) return -1;
-    if (make_tmap_heads(&a.tmK, k, D, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, ATTN_KV_BOX_ROWS)) return -1;
-    const int dvpad = (dv + 63) / 64 * 64;
-    if (make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, D, (int64_t)Nk * D, (int64_t)H * Nk * D, ATTN_KV_BOX_ROWS)) return -1;
-    a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk;
-    a.dqk_slabs = Dpad / 64;
-    a.dv_slabs = dvpad / 64;
-    a.dv = dv;
-    a.dqk = D;
-    a.scale_log2 = scale * 1.4426950408889634f;
-    a.out = out;
-    a.ldo = H * D;
-    a.out_col0 = v0;
-    a.out_hstride = D;  // heads are interleaved in the output as h*D + j, whatever slice of the value dim a pass covers
-    rc = attention_launch(a, bf16, stream);
-    count_launch();
-  }
-  return rc;
+  // [B, H, N, D] contiguous; heads are interleaved in the output as h*D + j
+  const int64_t sq = (int64_t)Nq * D, sk = (int64_t)Nk * D;
+  std::vector<AttnArgs> passes;
+  if (attention_args(passes, {q, D, sq, H * sq}, {k, D, sk, H * sk}, {v, D, sk, H * sk}, B, H, Nq, Nk, D, D, scale, out,
+                     H * D, D))
+    return -1;
+  for (const AttnArgs& a : passes)
+    if (int rc = attention_launch(a, dtype == SDXE_BF16, stream)) return rc;
+  return 0;
 }
 
 int sdxe_gemm(const void* A, const void* W, void* out, int M, int N, int K, const float* bias, const void* residual,
@@ -57,63 +40,40 @@ int sdxe_gemm(const void* A, const void* W, void* out, int M, int N, int K, cons
   const bool bf16 = dtype == SDXE_BF16;
   const bool geglu = flags & 1;
   void* scratch = nullptr;
-  const void* Wp = W;
-  const float* bp = bias;
-  GemmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.M = M; a.N = N; a.K = K; a.K1 = K;
-  a.epi = geglu ? EPI_GEGLU : EPI_PLAIN;
-  a.BN = gemm_pick_bn(M, N, K, a.epi);
-  if (flags >> 8) a.BN = flags >> 8;  // test hook: force the tile width
+  GemmW w;
+  w.w = W; w.rows = N; w.ld = K; w.N = N; w.K = K; w.bias = bias;
   if (geglu) {
-    // interleave value / gate rows per tile so that both land in the same accumulator tile
+    // value / gate rows interleaved per tile, so that both land in the same accumulator tile (packed below, once the
+    // tile width is chosen)
     SDXE_CUDA_CHECK(cudaMallocAsync(&scratch, (size_t)N * K * 2 + (size_t)N * 4, stream));
-    if (pack_weight_launch(W, dtype, scratch, PACK_GEGLU, N, K, K, a.BN, bf16, stream)) { cudaFreeAsync(scratch, stream); return -1; }
-    Wp = scratch;
-    if (bias) {
-      float* b2 = (float*)((char*)scratch + (size_t)N * K * 2);
-      if (pack_vector_launch(bias, SDXE_F32, b2, N, a.BN, false, bf16, stream)) { cudaFreeAsync(scratch, stream); return -1; }
-      bp = b2;
-    }
+    w.w = scratch;
+    if (bias) w.bias = (const float*)((char*)scratch + (size_t)N * K * 2);
   }
-  if (make_tmap_2d(&a.tmA, A, M, K, K, 128)) { if (scratch) cudaFreeAsync(scratch, stream); return -1; }
-  a.tmA2 = a.tmA;
-  a.bias = bp;
-  a.residual = residual;
-  a.ldr = N;
-  a.out = out;
-  a.ldo = geglu ? N / 2 : N;
-  a.rows_per_sample = 1;
-  if (gemm_finish_args(a, Wp, N, K)) { if (scratch) cudaFreeAsync(scratch, stream); return -1; }
-  int rc = gemm_launch(a, bf16, stream);
-  count_launch();
+  GemmEpi o;
+  o.epi = geglu ? EPI_GEGLU : EPI_PLAIN;
+  o.residual = residual;
+  o.ldr = N;
+  GemmArgs a;
+  int rc = gemm_args(a, GemmA::matrix(A, M, K), w, out, o, flags >> 8);  // flags >> 8: test hook forcing the tile width
+  if (rc == 0 && geglu) {
+    rc = pack_weight_launch(W, dtype, scratch, PACK_GEGLU, N, K, K, a.BN, bf16, stream);
+    if (rc == 0 && bias) rc = pack_vector_launch(bias, SDXE_F32, (float*)w.bias, N, a.BN, false, bf16, stream);
+  }
+  if (rc == 0) rc = gemm_launch(a, bf16, stream);
   if (scratch) cudaFreeAsync(scratch, stream);
   return rc;
 }
 
 int sdxe_conv3x3_nhwc(const void* x, const void* w, void* out, int n, int h, int wd, int cin, int cout,
                       const float* bias, int dtype, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (!is16(dtype) || cin % 64 || cout % 8) { set_last_error(__FILE__, __LINE__, "sdxe_conv3x3: alignment"); return -2; }
-  const bool bf16 = dtype == SDXE_BF16;
   int bw, bh, bn;
+  if (!is16(dtype) || cin % 64 || cout % 8) { set_last_error(__FILE__, __LINE__, "sdxe_conv3x3: alignment"); return -2; }
   if (!conv_tile_shape(h, wd, &bw, &bh, &bn)) { set_last_error(__FILE__, __LINE__, "sdxe_conv3x3: unsupported H x W tile"); return -2; }
+  GemmW W;
+  W.w = w; W.rows = cout; W.ld = 9 * cin; W.N = cout; W.K = 9 * cin; W.bias = bias;
   GemmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.M = n * h * wd; a.N = cout; a.K = 9 * cin; a.K1 = a.K;
-  a.conv = 1; a.cblocks = cin / 64; a.H = h; a.W = wd; a.bh = bh; a.bn = bn;
-  a.epi = EPI_PLAIN;
-  a.BN = gemm_pick_bn(a.M, a.N, a.K, a.epi);
-  if (make_tmap_nhwc(&a.tmA, x, n, h, wd, cin, bw, bh, bn)) return -1;
-  a.tmA2 = a.tmA;
-  a.bias = bias;
-  a.out = out;
-  a.ldo = cout;
-  a.rows_per_sample = 1;
-  if (gemm_finish_args(a, w, cout, a.K)) return -1;
-  int rc = gemm_launch(a, bf16, stream);
-  count_launch();
-  return rc;
+  if (gemm_args(a, GemmA::nhwc(x, n, h, wd, cin), W, out, GemmEpi())) return -1;
+  return gemm_launch(a, dtype == SDXE_BF16, (cudaStream_t)stream_);
 }
 
 int sdxe_group_norm_nhwc(const void* x, const float* gamma, const float* beta, void* out, int n, int hw, int c,
@@ -144,7 +104,6 @@ int sdxe_cfg_combine(const float* x, const void* eps, const float* sigma, float 
 int sdxe_lincomb(float* out, const float* p0, float c0, const float* p1, float c1, const float* p2, float c2, const float* p3,
                  float c3, int64_t total, void* stream) {
   if (!out || !p0 || total < 0) { set_last_error(__FILE__, __LINE__, "sdxe_lincomb: bad argument"); return -1; }
-  count_launch();
   return lincomb_launch(out, p0, c0, p1, c1, p2, c2, p3, c3, total, (cudaStream_t)stream);
 }
 int sdxe_cfg_combine_multi(const float* x, const void* eps, const float* sigma, const int32_t* row_ptr,

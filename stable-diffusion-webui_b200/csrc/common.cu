@@ -1,13 +1,17 @@
-// Host-side helpers: last-error string, TMA tensor-map encoding via the driver entry point, device query.
+// Host-side helpers: last-error string, launch counter, TMA tensor-map encoding via the driver entry point, device query.
 #include "common.cuh"
-#include <cstdlib>
 #include <cstdio>
 #include <cstring>
+#include <atomic>
 #include <mutex>
 
 namespace sdxe {
 
 static thread_local char g_err[1024] = "";
+static std::atomic<int64_t> g_launches{0};
+
+void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
 
 void set_last_error(const char* file, int line, const char* msg) {
   snprintf(g_err, sizeof(g_err), "%s:%d: %s", file, line, msg);
@@ -32,12 +36,12 @@ static PFN_encodeTiled get_encode() {
 }
 
 static int encode(CUtensorMap* out, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
-                  const cuuint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+                  const cuuint32_t* box) {
   PFN_encodeTiled fn = get_encode();
   if (!fn) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return -1; }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[256];
@@ -49,13 +53,6 @@ static int encode(CUtensorMap* out, const void* base, int rank, const cuuint64_t
   return 0;
 }
 
-bool pdl_enabled() {
-  static int v = -1;
-  // default off: the plans are replayed as CUDA graphs, which already hide most launch latency
-  if (v < 0) { const char* e = getenv("SDXE_PDL"); v = e ? atoi(e) : 0; }
-  return v != 0;
-}
-
 int make_tmap_2d(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
@@ -63,15 +60,6 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int64_t rows, int64_t cols,
   return encode(out, base, 2, dims, strides, box);
 }
 
-int make_tmap_2d_box(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  const CUtensorMapSwizzle sw = box_cols * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                              : box_cols * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                              : box_cols * 2 == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
-  return encode(out, base, 2, dims, strides, box, sw);
-}
 int make_tmap_heads(CUtensorMap* out, const void* base, int64_t d, int64_t tokens, int64_t heads, int64_t batch,
                     int64_t tok_stride, int64_t head_stride, int64_t batch_stride, int box_rows) {
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)tokens, (cuuint64_t)heads, (cuuint64_t)batch};
@@ -79,14 +67,6 @@ int make_tmap_heads(CUtensorMap* out, const void* base, int64_t d, int64_t token
   cuuint32_t box[4] = {64, (cuuint32_t)box_rows, 1, 1};
   return encode(out, base, 4, dims, strides, box);
 }
-int make_tmap_3d(CUtensorMap* out, const void* base, int64_t d0, int64_t d1, int64_t d2, int64_t pitch1, int64_t pitch2,
-                 int box_rows) {
-  cuuint64_t dims[3] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2};
-  cuuint64_t strides[2] = {(cuuint64_t)pitch1 * 2, (cuuint64_t)pitch2 * 2};
-  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
-  return encode(out, base, 3, dims, strides, box);
-}
-
 int make_tmap_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int bw, int bh, int bn) {
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};

@@ -74,14 +74,6 @@ SDXE_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// Programmatic dependent launch (PDL). A kernel launched through launch_k() may start while its predecessor in the
-// stream is still draining: everything before pdl_wait() (smem carve-up, mbarrier init, tensor-map
-// prefetch) overlaps the predecessor's tail; pdl_wait() returns once the predecessor grid has completed and its writes
-// are visible, so NO global memory may be read or written before it. pdl_launch_dependents() lets the successor
-// begin launching once every CTA of this grid has started. Both are no-ops for a normally launched kernel.
-SDXE_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-SDXE_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 // Non-blocking probe of a phase (for a consumer that serves several producers in arrival order).
 SDXE_DEVINL bool mbar_test(uint32_t bar, uint32_t parity) {
   uint32_t done;
@@ -276,38 +268,25 @@ const char* last_error();
 
 // 16-bit row-major 2D [rows, cols] with row pitch ld (elements): box = 64 cols x box_rows, 128B swizzle.
 int make_tmap_2d(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
-// same with an explicit box; swizzle = the box's row bytes (32 / 64 / 128 B) — the GEMM epilogue's store / residual boxes
-int make_tmap_2d_box(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows);
 // per-head view of a row-major activation: element (j, tok, h, b) at base + b*batch_stride + tok*tok_stride + h*head_stride
 // + j (strides in elements, multiples of 8). Inner extent d (NOT padded): a 64-wide box past d is zero-filled by TMA.
 int make_tmap_heads(CUtensorMap* out, const void* base, int64_t d, int64_t tokens, int64_t heads, int64_t batch,
                     int64_t tok_stride, int64_t head_stride, int64_t batch_stride, int box_rows);
-// 16-bit 3D [d2, d1 rows, d0 cols] with pitches: box = 64 x box_rows x 1.
-int make_tmap_3d(CUtensorMap* out, const void* base, int64_t d0, int64_t d1, int64_t d2, int64_t pitch1, int64_t pitch2,
-                 int box_rows);
 // 16-bit NHWC activations [N, H, W, C]: box = 64 ch x bw x bh x bn, 128B swizzle, OOB -> zero (= conv padding).
 int make_tmap_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int bw, int bh, int bn);
 int make_tmap_nhwc_s2(CUtensorMap* out, const void* base, int N, int H, int W, int C, int bw, int bh, int bn);
 
 int num_sms();
-bool pdl_enabled();  // SDXE_PDL=1 turns programmatic dependent launch on (default off)
 
-// Launch with the programmatic-stream-serialization attribute (see pdl_wait above). Only for kernels that call
-// pdl_wait() before touching global memory.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
+// Kernels launched by this library (sdxe_launch_count). Every launch site counts itself once, through SDXE_LAUNCH_CHECK;
+// a replayed CUDA graph adds the count its capture recorded.
+void count_launch(int n = 1);
+int64_t launch_count();
+
+#define SDXE_LAUNCH_CHECK()                 \
+  do {                                      \
+    ::sdxe::count_launch();                 \
+    SDXE_CUDA_CHECK(cudaGetLastError());    \
+  } while (0)
 
 }  // namespace sdxe

@@ -65,8 +65,14 @@ struct ResW {
   LinW c1, c2, skip;
   bool has_skip = false;
   int cin = 0, cout = 0;
-  int emb_off = -1;  // column offset into the batched emb_layers output
+  int emb_off = -1;  // UNet: column offset into the batched emb_layers output
 };
+// state-dict names of a ResBlock's layers, relative to the block
+struct ResKeys {
+  const char *n1, *c1, *n2, *c2, *skip;
+};
+const ResKeys UNET_RES = {".in_layers.0", ".in_layers.2", ".out_layers.0", ".out_layers.3", ".skip_connection"};
+const ResKeys VAE_RES = {".norm1", ".conv1", ".norm2", ".conv2", ".nin_shortcut"};
 struct TBlockW {
   NormW ln1, ln2, ln3;
   LinW qkv1, out1, q2, out2, ff1, ff2;
@@ -88,12 +94,6 @@ struct BlockW {  // one TimestepEmbedSequential
   LinW down;  // Downsample.op
   LinW conv_in;
   int ch_out = 0;
-};
-struct VaeResW {
-  NormW n1, n2;
-  LinW c1, c2, skip;
-  bool has_skip = false;
-  int cin = 0, cout = 0;
 };
 
 struct ClipLayerW {  // CLIPEncoderLayer: LN1 -> q|k|v -> causal attention -> out_proj (+x) -> LN2 -> fc1 -> act -> fc2 (+x)
@@ -147,14 +147,14 @@ struct sdxe_engine {
   float* pq_w = nullptr;  // post_quant_conv [z, z] fp32
   float* pq_b = nullptr;
   LinW v_conv_in, v_conv_out, v_qkv, v_proj;
-  VaeResW v_mid1, v_mid2;
+  ResW v_mid1, v_mid2;
   NormW v_attn_norm, v_norm_out;
-  std::vector<std::vector<VaeResW>> v_up_blocks;  // [level][block], level index as in the state dict
+  std::vector<std::vector<ResW>> v_up_blocks;  // [level][block], level index as in the state dict
   // VAE encoder (ldm Encoder: conv_in, down.{l}.block.{j} (+ downsample), mid, norm_out, conv_out; then quant_conv)
   LinW e_conv_in, e_conv_out, e_qkv, e_proj, e_quant;
-  VaeResW e_mid1, e_mid2;
+  ResW e_mid1, e_mid2;
   NormW e_attn_norm, e_norm_out;
-  std::vector<std::vector<VaeResW>> e_down_blocks;
+  std::vector<std::vector<ResW>> e_down_blocks;
   std::vector<LinW> e_down_conv;
   std::vector<LinW> v_up_conv;                    // per level (level 0 unused)
   // CLIP text transformer
@@ -176,14 +176,13 @@ struct sdxe_engine {
   // same key skips the context cast + projection GEMM (modules/sd_samplers_cfg_denoiser.py re-sends the same cond_in
   // every sampler step).
   int64_t ctx_key = 0;
-  int max_plans = 8;                    // SDXE_MAX_PLANS
-  size_t pool_limit = (size_t)6 << 30;  // SDXE_POOL_LIMIT_MB: free (unowned) pool bytes kept after an eviction
+  int max_plans = 8;                    // sdxe_set_plan_cache
+  size_t pool_limit = (size_t)6 << 30;  // free (unowned) pool bytes kept after an eviction (sdxe_set_plan_cache)
   uint64_t tick = 0;
   std::vector<Buf>* track = nullptr;    // while a plan is being built: the buffers it currently holds
   std::vector<void*>* touched = nullptr;  // ... and every pool block it used at any point (scratch it released again)
   bool alloc_failed = false;
   cudaStream_t cap_stream = nullptr;
-  bool use_graph = true;
   bool profiling = false;
   double prof_ms[8] = {0}, prof_flops[8] = {0}, prof_bytes[8] = {0};
   int64_t prof_launches[8] = {0};
@@ -202,9 +201,8 @@ struct sdxe_engine {
   int build_vae();
   int build_vae_encoder();
   int build_clip();
-  int build_res(ResW& r, const std::string& p, int cin, int cout);
+  int build_res(ResW& r, const std::string& p, int cin, int cout, const ResKeys& k);
   int build_st(STW& s, const std::string& p, int C, int depth);
-  int build_vae_res(VaeResW& r, const std::string& p, int cin, int cout);
   // --- activations
   Buf alloc(size_t bytes);
   void release(Buf& b);
@@ -281,135 +279,82 @@ struct Builder {
     st.p = nullptr; st.parts = 0;
   }
   // out[M, N] = A (+A2) * W^T with the fused epilogues of gemm.cu
-  struct GemmOpt {
+  struct GemmOpt : GemmEpi {
     const void* A2 = nullptr;
     int K1 = 0;            // columns taken from A (A2 supplies K - K1)
-    const float* rowvec = nullptr;
-    int ldrv = 0, rows_per_sample = 1;
-    const void* residual = nullptr;
-    int ldr = 0;
-    int epi = EPI_PLAIN;
-    int ldo = 0;
-    // LayerNorm fold (gemm.cuh): statistics of the A rows as emitted by the GEMM that produced A
-    const float2* ln_part = nullptr;
-    int ln_parts = 0;
     // emit per-row partial statistics of the output for a following folded LayerNorm: filled in by gemm()
     RowStats* emit = nullptr;
   };
+  static GemmW weight(const LinW& W) {
+    GemmW w;
+    w.w = W.w; w.rows = std::max(W.N, W.Nrows); w.ld = W.ld; w.N = W.N; w.K = W.K; w.bias = W.b; w.c1 = W.c1;
+    return w;
+  }
   int gemm(const void* A, int lda, int64_t M, const LinW& W, void* out, const GemmOpt& o) {
+    GemmEpi epi = o;
+    if (o.emit)
+      epi.stat_out = [this, M, st = o.emit](int parts) {
+        st->buf = e->alloc((size_t)parts * M * sizeof(float2));
+        st->p = (const float2*)st->buf.p;
+        st->parts = parts;
+        return (float2*)st->buf.p;
+      };
     GemmArgs a;
-    memset(&a, 0, sizeof(a));
-    a.M = (int)M; a.N = W.N; a.K = W.K;
-    a.K1 = o.A2 ? o.K1 : W.K;
-    a.epi = o.epi;
-    a.BN = (o.epi == EPI_GEGLU) ? W.geglu_tile : gemm_pick_bn(a.M, a.N, a.K, a.epi);
-    ECHK(make_tmap_2d(&a.tmA, A, M, a.K1, lda, 128));
-    if (o.A2) ECHK(make_tmap_2d(&a.tmA2, o.A2, M, W.K - o.K1, W.K - o.K1, 128));
-    else a.tmA2 = a.tmA;
-    a.bias = W.b;
-    a.rowvec = o.rowvec; a.ldrv = o.ldrv; a.rows_per_sample = std::max(1, o.rows_per_sample);
-    a.residual = o.residual; a.ldr = o.ldr;
-    a.out = out;
-    a.ldo = o.ldo ? o.ldo : (o.epi == EPI_GEGLU ? W.N / 2 : (W.N + 7) / 8 * 8);
-    if (W.c1) {  // this weight has a LayerNorm folded in: it can only be applied with the row statistics of A
-      if (!o.ln_part || o.A2) EFAIL("gemm: folded LayerNorm weight without row statistics");
-      a.c1 = W.c1; a.ln_part = o.ln_part; a.ln_parts = o.ln_parts;
-      a.ln_inv_c = 1.0f / (float)W.K; a.ln_eps = 1e-5f;
-    }
-    if (o.emit) {
-      const int num_n = (a.N + a.BN - 1) / a.BN;
-      o.emit->buf = e->alloc((size_t)num_n * M * sizeof(float2));
-      o.emit->p = (const float2*)o.emit->buf.p;
-      o.emit->parts = num_n;
-      a.stat_out = (float2*)o.emit->buf.p;
-    }
-    ECHK(gemm_finish_args(a, W.w, std::max(W.N, W.Nrows), W.ld));
+    ECHK(gemm_args(a, GemmA::matrix(A, M, lda, o.A2, o.K1), weight(W), out, epi, o.epi == EPI_GEGLU ? W.geglu_tile : 0));
     const bool b = bf16;
     const double nout = (o.epi == EPI_GEGLU) ? W.N / 2.0 : (double)W.N;
     const double by = 2.0 * ((double)M * W.K + (double)W.N * W.K + (double)M * nout + (o.residual ? (double)M * nout : 0.0));
     char d[160];
     snprintf(d, sizeof(d), "gemm M=%lld N=%d K=%d BN=%d st=%d epi=%d res=%d rv=%d dual=%d", (long long)M, W.N, W.K, a.BN, a.num_stages, o.epi,
              o.residual ? 1 : 0, o.rowvec ? 1 : 0, o.A2 ? 1 : 0);
-    ops->push_back(OpRec([a, b](cudaStream_t s) { count_launch(); return gemm_launch(a, b, s); }, K_GEMM,
-                         2.0 * (double)M * W.N * W.K, by, d));
+    ops->push_back(OpRec([a, b](cudaStream_t s) { return gemm_launch(a, b, s); }, K_GEMM, 2.0 * (double)M * W.N * W.K, by, d));
     return 0;
   }
 
-  // 3x3 stride-1 pad-1 conv of an NHWC activation; W packed [Cout, 9*Cin (ld)]
-  int conv3(const Act& x, const LinW& W, void* out, int ldo, const GemmOpt& o) {
+  // 3x3 conv of an NHWC activation, W packed [Cout, 9*Cin (ld)]: stride 1 pad 1, or stride 2 (ldm Downsample) with pad_lo
+  // zero rows / columns before the image and output Ho x Wo. Implicit GEMM when the geometry allows it, else im2col.
+  int conv3(const Act& x, const LinW& W, void* out, int ldo, const GemmOpt& o, int stride = 1, int pad_lo = 1, int Ho = 0,
+            int Wo = 0) {
+    static int s2_implicit = -1;
+    if (s2_implicit < 0) { const char* ev = getenv("SDXE_CONV_S2_IMPLICIT"); s2_implicit = ev ? atoi(ev) : 1; }
+    if (stride == 1) { Ho = x.h; Wo = x.w; }
     int bw, bh, bn;
-    if (x.c % 64 == 0 && conv_tile_shape(x.h, x.w, &bw, &bh, &bn)) {
-      GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      a.M = (int)x.rows(); a.N = W.N; a.K = 9 * x.c; a.K1 = a.K;
-      a.conv = 1; a.cblocks = x.c / 64; a.H = x.h; a.W = x.w; a.bh = bh; a.bn = bn;
-      a.epi = EPI_PLAIN;
-      a.BN = gemm_pick_bn(a.M, a.N, a.K, a.epi);
-      ECHK(make_tmap_nhwc(&a.tmA, x.p, x.n, x.h, x.w, x.c, bw, bh, bn));
-      a.tmA2 = a.tmA;
-      a.bias = W.b;
-      a.rowvec = o.rowvec; a.ldrv = o.ldrv; a.rows_per_sample = std::max(1, o.rows_per_sample);
-      a.residual = o.residual; a.ldr = o.ldr;
-      a.out = out; a.ldo = ldo;
-      ECHK(gemm_finish_args(a, W.w, std::max(W.N, W.Nrows), W.ld));
+    const bool implicit = x.c % 64 == 0 && W.ld == 9 * x.c && conv_tile_shape(Ho, Wo, &bw, &bh, &bn) &&
+                          (stride == 1 || (s2_implicit && x.h % 2 == 0 && x.w % 2 == 0 && Ho == x.h / 2 && Wo == x.w / 2));
+    if (!implicit) {  // generic geometry: explicit im2col (still CUDA; used for odd resolutions / narrow channel counts)
+      const int kpad = W.ld;
+      const int64_t M = (int64_t)x.n * Ho * Wo;
+      Buf col = e->alloc((size_t)M * kpad * 2);
+      const void* xp = x.p;
+      void* cp = col.p;
+      const int n = x.n, H = x.h, Wd = x.w, C = x.c;
       const bool b = bf16;
-      const double Md = (double)a.M;
-      const double by = 2.0 * (Md * x.c + (double)W.N * a.K + Md * W.N + (o.residual ? Md * W.N : 0.0));
-      char d[160];
+      ops->push_back([=](cudaStream_t s) { return im2col3x3_launch(xp, cp, n, H, Wd, C, Ho, Wo, stride, pad_lo, kpad, b, s); });
+      LinW W2 = W;
+      W2.K = kpad;  // zero-padded columns on both sides
+      GemmOpt o2 = o;
+      o2.ldo = ldo;
+      ECHK(gemm(col.p, kpad, M, W2, out, o2));
+      e->release(col);
+      return 0;
+    }
+    GemmEpi epi = o;
+    epi.ldo = ldo;
+    GemmArgs a;
+    ECHK(gemm_args(a, GemmA::nhwc(x.p, x.n, x.h, x.w, x.c, stride, pad_lo), weight(W), out, epi));
+    const bool b = bf16;
+    const double Md = (double)a.M;
+    char d[160];
+    double by;
+    if (stride == 1) {
+      by = 2.0 * (Md * x.c + (double)W.N * a.K + Md * W.N + (o.residual ? Md * W.N : 0.0));
       snprintf(d, sizeof(d), "conv3 M=%d N=%d Cin=%d HxW=%dx%d BN=%d st=%d res=%d rv=%d", a.M, W.N, x.c, x.h, x.w, a.BN, a.num_stages,
                o.residual ? 1 : 0, o.rowvec ? 1 : 0);
-      ops->push_back(OpRec([a, b](cudaStream_t s) { count_launch(); return gemm_launch(a, b, s); }, K_CONV,
-                           2.0 * Md * W.N * a.K, by, d));
-      return 0;
-    }
-    // generic geometry: explicit im2col (still CUDA; used for odd resolutions / narrow channel counts)
-    return conv3_im2col(x, W, out, ldo, o, 1, 1, x.h, x.w);
-  }
-  // 3x3 stride-2 conv (ldm Downsample): implicit GEMM over the pixel-pair view when the geometry allows it
-  int conv3_s2(const Act& x, const LinW& W, void* out, int ldo, const GemmOpt& o, int pad_lo, int Ho, int Wo) {
-    int bw, bh, bn;
-    static int implicit = -1;
-    if (implicit < 0) { const char* ev = getenv("SDXE_CONV_S2_IMPLICIT"); implicit = ev ? atoi(ev) : 1; }
-    if (implicit && x.c % 64 == 0 && x.h % 2 == 0 && x.w % 2 == 0 && Ho == x.h / 2 && Wo == x.w / 2 && W.ld == 9 * x.c &&
-        conv_tile_shape(Ho, Wo, &bw, &bh, &bn)) {
-      GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      a.M = x.n * Ho * Wo; a.N = W.N; a.K = 9 * x.c; a.K1 = a.K;
-      a.conv = 2; a.pad_lo = pad_lo; a.cblocks = x.c / 64; a.H = Ho; a.W = Wo; a.bh = bh; a.bn = bn;
-      a.epi = EPI_PLAIN;
-      a.BN = gemm_pick_bn(a.M, a.N, a.K, a.epi);
-      ECHK(make_tmap_nhwc_s2(&a.tmA, x.p, x.n, x.h, x.w, x.c, bw, bh, bn));
-      a.tmA2 = a.tmA;
-      a.bias = W.b;
-      a.rowvec = o.rowvec; a.ldrv = o.ldrv; a.rows_per_sample = std::max(1, o.rows_per_sample);
-      a.residual = o.residual; a.ldr = o.ldr;
-      a.out = out; a.ldo = ldo;
-      ECHK(gemm_finish_args(a, W.w, std::max(W.N, W.Nrows), W.ld));
-      const bool b = bf16;
-      const double Md = (double)a.M;
-      const double by = 2.0 * (4.0 * Md * x.c + (double)W.N * a.K + Md * W.N);
-      char d[160];
+    } else {
+      by = 2.0 * (4.0 * Md * x.c + (double)W.N * a.K + Md * W.N);
       snprintf(d, sizeof(d), "conv3s2 M=%d N=%d Cin=%d HoxWo=%dx%d BN=%d st=%d", a.M, W.N, x.c, Ho, Wo, a.BN, a.num_stages);
-      ops->push_back(OpRec([a, b](cudaStream_t s) { count_launch(); return gemm_launch(a, b, s); }, K_CONV, 2.0 * Md * W.N * a.K, by, d));
-      return 0;
     }
-    return conv3_im2col(x, W, out, ldo, o, 2, pad_lo, Ho, Wo);
-  }
-  int conv3_im2col(const Act& x, const LinW& W, void* out, int ldo, const GemmOpt& o, int stride, int pad_lo, int Ho, int Wo) {
-    const int kpad = W.ld;
-    const int64_t M = (int64_t)x.n * Ho * Wo;
-    Buf col = e->alloc((size_t)M * kpad * 2);
-    const void* xp = x.p;
-    void* cp = col.p;
-    const int n = x.n, H = x.h, Wd = x.w, C = x.c;
-    const bool b = bf16;
-    ops->push_back([=](cudaStream_t s) { return im2col3x3_launch(xp, cp, n, H, Wd, C, Ho, Wo, stride, pad_lo, kpad, b, s); });
-    LinW W2 = W;
-    W2.K = kpad;  // zero-padded columns on both sides
-    GemmOpt o2 = o;
-    o2.ldo = ldo;
-    ECHK(gemm(col.p, kpad, M, W2, out, o2));
-    e->release(col);
+    ops->push_back(OpRec([a, b](cudaStream_t s) { return gemm_launch(a, b, s); }, K_CONV, 2.0 * Md * W.N * a.K, by, d));
     return 0;
   }
 
@@ -430,50 +375,89 @@ struct Builder {
     return 0;
   }
   // q: [B*Nq, ldq], k / v: [B*Nk, ldkv] row-major activations whose columns h*d .. h*d+d-1 belong to head h (the
-  // projection GEMM's natural output). The kernels see them through 4D tensor maps (d, token, head, batch); a 64-wide
-  // box reaching past d is zero-filled by TMA, so no padded per-head copy exists.
+  // projection GEMM's natural output), seen through per-head views: no padded per-head copy exists.
   int attention(const void* q, const void* k, const void* v, int B, int H, int Nq, int Nk, int d, int ldq, int ldkv,
                 float scale, void* out, int ldo, int dv_total) {
+    std::vector<AttnArgs> passes;
+    const AttnView vq = {q, ldq, d, (int64_t)Nq * ldq}, vk = {k, ldkv, d, (int64_t)Nk * ldkv}, vv = {v, ldkv, d, (int64_t)Nk * ldkv};
+    ECHK(attention_args(passes, vq, vk, vv, B, H, Nq, Nk, d, dv_total, scale, out, ldo, dv_total));
     const int dpad = (d + 63) / 64 * 64;
-    // value columns in passes of at most ATTN_MAX_DV (VAE d = 512, SD1.5 d = 160)
-    for (int v0 = 0; v0 < dv_total; v0 += ATTN_MAX_DV) {
-      const int dv = std::min(ATTN_MAX_DV, dv_total - v0);
-      const int dvpad = (dv + 63) / 64 * 64;
-      AttnArgs a;
-      memset(&a, 0, sizeof(a));
-      ECHK(make_tmap_heads(&a.tmQ, q, d, Nq, H, B, ldq, d, (int64_t)Nq * ldq, ATTN_Q_BOX_ROWS));
-      ECHK(make_tmap_heads(&a.tmK, k, d, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, ATTN_KV_BOX_ROWS));
-      ECHK(make_tmap_heads(&a.tmV, (const uint16_t*)v + v0, dv, Nk, H, B, ldkv, d, (int64_t)Nk * ldkv, ATTN_KV_BOX_ROWS));
-      a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk;
-      a.dqk_slabs = dpad / 64;
-      a.dv_slabs = dvpad / 64;
-      a.dv = dv;
-      a.dqk = d;
-      a.out_hstride = dv_total;
-      a.scale_log2 = scale * 1.4426950408889634f;
-      a.out = out; a.ldo = ldo; a.out_col0 = v0;
+    for (const AttnArgs& a : passes) {  // value columns in passes (VAE d = 512, SD1.5 d = 160)
+      const int dv = a.dv;
       const bool b = bf16;
       const double fl = 2.0 * (double)B * H * Nq * Nk * ((double)d + dv);
       const double by = 2.0 * (double)B * H * ((double)Nq * d + (double)Nk * (d + dv) + (double)Nq * dv);
       char dsc[160];
       snprintf(dsc, sizeof(dsc), "attn B=%d H=%d Nq=%d Nk=%d d=%d dpad=%d dv=%d", B, H, Nq, Nk, d, dpad, dv);
-      ops->push_back(OpRec([a, b](cudaStream_t s) { count_launch(); return attention_launch(a, b, s); }, K_ATTN, fl, by, dsc));
+      ops->push_back(OpRec([a, b](cudaStream_t s) { return attention_launch(a, b, s); }, K_ATTN, fl, by, dsc));
     }
     return 0;
   }
 
+  // 3x3 conv of the model's NCHW input: im2col3x3_nchw in `pre`, then the GEMM with K = ld. src: a plan buffer of the
+  // engine's dtype, or null for the caller's x (in its io dtype, read at run time).
+  int conv_in_nchw(const void* src, int n, int c, int h, int w, const LinW& W, Act& out) {
+    const int kin = W.ld;
+    Buf col = e->alloc((size_t)n * h * w * kin * 2);  // plan-owned
+    {
+      Plan* p = plan;
+      void* cp = col.p;
+      const int edt = e->dt;
+      const bool b = bf16;
+      plan->pre.push_back([=](cudaStream_t s) {
+        return im2col3x3_nchw_launch(src ? src : p->x, src ? edt : p->io_dtype, cp, n, c, h, w, kin, b, s);
+      });
+    }
+    out = new_act(n, h, w, W.N);
+    LinW Wk = W;
+    Wk.K = kin;
+    return gemm(col.p, kin, out.rows(), Wk, out.p, GemmOpt());
+  }
+  // ldm Upsample: nearest 2x, then 3x3 conv; x is released
+  int upsample_conv(Act& x, const LinW& W, Act& out) {
+    Act up = new_act(x.n, x.h * 2, x.w * 2, x.c);
+    {
+      const void* xp = x.p;
+      void* upp = up.p;
+      const int n = x.n, h = x.h, w = x.w, c = x.c;
+      ops->push_back([=](cudaStream_t s) { return upsample2x_launch(xp, upp, n, h, w, c, s); });
+    }
+    free_act(x);
+    out = new_act(up.n, up.h, up.w, up.c);
+    ECHK(conv3(up, W, out.p, up.c, GemmOpt()));
+    free_act(up);
+    return 0;
+  }
+  // output head: GroupNorm + SiLU -> 3x3 conv -> the caller's NCHW output (in `post`); x is released
+  int out_head(Act& x, const NormW& norm, float eps, const LinW& W) {
+    Act g;
+    ECHK(group_norm(x, nullptr, norm, eps, true, g));
+    free_act(x);
+    const int ldo = (int)align_up(W.N, 8);
+    Buf outb = e->alloc((size_t)g.rows() * ldo * 2);  // plan-owned
+    ECHK(conv3(g, W, outb.p, ldo, GemmOpt()));
+    free_act(g);
+    Plan* p = plan;
+    void* ob = outb.p;
+    const int n = g.n, oc = W.N, hw = g.h * g.w;
+    const bool b = bf16;
+    plan->post.push_back([=](cudaStream_t s) { return nhwc_to_nchw_launch(ob, ldo, p->out, p->io_dtype, n, oc, hw, b, s); });
+    return 0;
+  }
+
   // ---- UNet building blocks --------------------------------------------------------------------------------
-  // ResBlock (ldm openaimodel.ResBlock): GN32+SiLU -> conv3 (+emb) -> GN32+SiLU -> conv3 (+skip)
-  int res_block(const ResW& r, Act& x, Act* skip_src, const float* emb_all, int ld_emb, Act& out) {
+  // ResBlock (ldm openaimodel.ResBlock, VAE ResnetBlock): GN32+SiLU -> conv3 (+emb) -> GN32+SiLU -> conv3 (+skip).
+  // emb_all: the UNet's batched timestep-embedding rows (null: none); skip_src: the UNet decoder's skip-concat input.
+  int res_block(const ResW& r, Act& x, Act* skip_src, const float* emb_all, int ld_emb, float eps, Act& out) {
     Act g1;
-    ECHK(group_norm(x, skip_src, r.n1, 1e-5f, true, g1));
+    ECHK(group_norm(x, skip_src, r.n1, eps, true, g1));
     Act h = new_act(x.n, x.h, x.w, r.cout);
     GemmOpt o1;
-    o1.rowvec = emb_all + r.emb_off; o1.ldrv = ld_emb; o1.rows_per_sample = x.h * x.w;
+    if (emb_all) { o1.rowvec = emb_all + r.emb_off; o1.ldrv = ld_emb; o1.rows_per_sample = x.h * x.w; }
     ECHK(conv3(g1, r.c1, h.p, r.cout, o1));
     free_act(g1);
     Act g2;
-    ECHK(group_norm(h, nullptr, r.n2, 1e-5f, true, g2));
+    ECHK(group_norm(h, nullptr, r.n2, eps, true, g2));
     free_act(h);
     Act sk;
     const void* res_ptr;
@@ -571,31 +555,6 @@ struct Builder {
     op.residual = x.p; op.ldr = C;
     ECHK(gemm(h.p, C, M, st.proj_out, out.p, op));
     free_act(h);
-    return 0;
-  }
-
-  int vae_res(const VaeResW& r, Act& x, Act& out) {
-    Act g1;
-    ECHK(group_norm(x, nullptr, r.n1, 1e-6f, true, g1));
-    Act h = new_act(x.n, x.h, x.w, r.cout);
-    ECHK(conv3(g1, r.c1, h.p, r.cout, GemmOpt()));
-    free_act(g1);
-    Act g2;
-    ECHK(group_norm(h, nullptr, r.n2, 1e-6f, true, g2));
-    free_act(h);
-    Act sk;
-    const void* res_ptr = x.p;
-    if (r.has_skip) {
-      sk = new_act(x.n, x.h, x.w, r.cout);
-      ECHK(gemm(x.p, x.c, x.rows(), r.skip, sk.p, GemmOpt()));
-      res_ptr = sk.p;
-    }
-    out = new_act(x.n, x.h, x.w, r.cout);
-    GemmOpt o2;
-    o2.residual = res_ptr; o2.ldr = r.cout;
-    ECHK(conv3(g2, r.c2, out.p, r.cout, o2));
-    free_act(g2);
-    if (r.has_skip) free_act(sk);
     return 0;
   }
 };
@@ -702,14 +661,15 @@ static int conv_kpad(int cin) {
   return (cin % 64 == 0) ? k : (int)align_up(k, 64);
 }
 
-int sdxe_engine::build_res(ResW& r, const std::string& p, int cin, int cout) {
+int sdxe_engine::build_res(ResW& r, const std::string& p, int cin, int cout, const ResKeys& k) {
   r.cin = cin; r.cout = cout;
-  ECHK(pack_norm(r.n1, p + ".in_layers.0", cin));
-  ECHK(pack_linear(r.c1, {p + ".in_layers.2.weight"}, {p + ".in_layers.2.bias"}, cout, 9 * cin, PACK_CONV3, conv_kpad(cin)));
-  ECHK(pack_norm(r.n2, p + ".out_layers.0", cout));
-  ECHK(pack_linear(r.c2, {p + ".out_layers.3.weight"}, {p + ".out_layers.3.bias"}, cout, 9 * cout, PACK_CONV3, conv_kpad(cout)));
+  const std::string c1 = p + k.c1, c2 = p + k.c2, sk = p + k.skip;
+  ECHK(pack_norm(r.n1, p + k.n1, cin));
+  ECHK(pack_linear(r.c1, {c1 + ".weight"}, {c1 + ".bias"}, cout, 9 * cin, PACK_CONV3, conv_kpad(cin)));
+  ECHK(pack_norm(r.n2, p + k.n2, cout));
+  ECHK(pack_linear(r.c2, {c2 + ".weight"}, {c2 + ".bias"}, cout, 9 * cout, PACK_CONV3, conv_kpad(cout)));
   r.has_skip = cin != cout;
-  if (r.has_skip) ECHK(pack_linear(r.skip, {p + ".skip_connection.weight"}, {p + ".skip_connection.bias"}, cout, cin, PACK_PLAIN));
+  if (r.has_skip) ECHK(pack_linear(r.skip, {sk + ".weight"}, {sk + ".bias"}, cout, cin, PACK_PLAIN));
   return 0;
 }
 
@@ -785,7 +745,7 @@ int sdxe_engine::build_unet() {
       BlockW b;
       b.kind = 1;
       const std::string p = "input_blocks." + std::to_string(idx);
-      ECHK(build_res(b.res, p + ".0", ch, mult * mc));
+      ECHK(build_res(b.res, p + ".0", ch, mult * mc, UNET_RES));
       add_emb(b.res, p + ".0");
       ch = mult * mc;
       if (cfg.transformer_depth[level] > 0) {
@@ -808,10 +768,10 @@ int sdxe_engine::build_unet() {
       ++idx;
     }
   }
-  ECHK(build_res(mid_r1, "middle_block.0", ch, ch));
+  ECHK(build_res(mid_r1, "middle_block.0", ch, ch, UNET_RES));
   add_emb(mid_r1, "middle_block.0");
   ECHK(build_st(mid_st, "middle_block.1", ch, std::max(1, cfg.transformer_depth_middle)));
-  ECHK(build_res(mid_r2, "middle_block.2", ch, ch));
+  ECHK(build_res(mid_r2, "middle_block.2", ch, ch, UNET_RES));
   add_emb(mid_r2, "middle_block.2");
   idx = 0;
   for (int level = nl - 1; level >= 0; --level) {
@@ -822,7 +782,7 @@ int sdxe_engine::build_unet() {
       BlockW b;
       b.kind = 1;
       const std::string p = "output_blocks." + std::to_string(idx);
-      ECHK(build_res(b.res, p + ".0", ch + ich, mc * mult));
+      ECHK(build_res(b.res, p + ".0", ch + ich, mc * mult, UNET_RES));
       add_emb(b.res, p + ".0");
       ch = mc * mult;
       int sub = 1;
@@ -875,36 +835,25 @@ int sdxe_engine::build_unet() {
   return 0;
 }
 
-int sdxe_engine::build_vae_res(VaeResW& r, const std::string& p, int cin, int cout) {
-  r.cin = cin; r.cout = cout;
-  ECHK(pack_norm(r.n1, p + ".norm1", cin));
-  ECHK(pack_linear(r.c1, {p + ".conv1.weight"}, {p + ".conv1.bias"}, cout, 9 * cin, PACK_CONV3, conv_kpad(cin)));
-  ECHK(pack_norm(r.n2, p + ".norm2", cout));
-  ECHK(pack_linear(r.c2, {p + ".conv2.weight"}, {p + ".conv2.bias"}, cout, 9 * cout, PACK_CONV3, conv_kpad(cout)));
-  r.has_skip = cin != cout;
-  if (r.has_skip) ECHK(pack_linear(r.skip, {p + ".nin_shortcut.weight"}, {p + ".nin_shortcut.bias"}, cout, cin, PACK_PLAIN));
-  return 0;
-}
-
 int sdxe_engine::build_vae() {
   const int z = cfg.vae_z_channels, nl = cfg.num_levels, nrb = cfg.num_res_blocks;
   ECHK(pack_f32(pq_w, "post_quant_conv.weight", (int64_t)z * z));
   ECHK(pack_f32(pq_b, "post_quant_conv.bias", z));
   int bi = cfg.vae_ch * cfg.channel_mult[nl - 1];
   ECHK(pack_linear(v_conv_in, {"decoder.conv_in.weight"}, {"decoder.conv_in.bias"}, bi, 9 * z, PACK_CONV3, conv_kpad(z)));
-  ECHK(build_vae_res(v_mid1, "decoder.mid.block_1", bi, bi));
+  ECHK(build_res(v_mid1, "decoder.mid.block_1", bi, bi, VAE_RES));
   ECHK(pack_norm(v_attn_norm, "decoder.mid.attn_1.norm", bi));
   ECHK(pack_linear(v_qkv, {"decoder.mid.attn_1.q.weight", "decoder.mid.attn_1.k.weight", "decoder.mid.attn_1.v.weight"},
                    {"decoder.mid.attn_1.q.bias", "decoder.mid.attn_1.k.bias", "decoder.mid.attn_1.v.bias"}, bi, bi, PACK_PLAIN));
   ECHK(pack_linear(v_proj, {"decoder.mid.attn_1.proj_out.weight"}, {"decoder.mid.attn_1.proj_out.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(build_vae_res(v_mid2, "decoder.mid.block_2", bi, bi));
+  ECHK(build_res(v_mid2, "decoder.mid.block_2", bi, bi, VAE_RES));
   v_up_blocks.assign(nl, {});
   v_up_conv.assign(nl, LinW());
   for (int level = nl - 1; level >= 0; --level) {
     const int bo = cfg.vae_ch * cfg.channel_mult[level];
     for (int j = 0; j <= nrb; ++j) {
-      VaeResW r;
-      ECHK(build_vae_res(r, "decoder.up." + std::to_string(level) + ".block." + std::to_string(j), bi, bo));
+      ResW r;
+      ECHK(build_res(r, "decoder.up." + std::to_string(level) + ".block." + std::to_string(j), bi, bo, VAE_RES));
       v_up_blocks[level].push_back(r);
       bi = bo;
     }
@@ -927,8 +876,8 @@ int sdxe_engine::build_vae_encoder() {
   for (int level = 0; level < nl; ++level) {
     const int bo = ch * cfg.channel_mult[level];
     for (int j = 0; j < nrb; ++j) {
-      VaeResW r;
-      ECHK(build_vae_res(r, "encoder.down." + std::to_string(level) + ".block." + std::to_string(j), bi, bo));
+      ResW r;
+      ECHK(build_res(r, "encoder.down." + std::to_string(level) + ".block." + std::to_string(j), bi, bo, VAE_RES));
       e_down_blocks[level].push_back(r);
       bi = bo;
     }
@@ -937,12 +886,12 @@ int sdxe_engine::build_vae_encoder() {
       ECHK(pack_linear(e_down_conv[level], {d + ".weight"}, {d + ".bias"}, bi, 9 * bi, PACK_CONV3, conv_kpad(bi)));
     }
   }
-  ECHK(build_vae_res(e_mid1, "encoder.mid.block_1", bi, bi));
+  ECHK(build_res(e_mid1, "encoder.mid.block_1", bi, bi, VAE_RES));
   ECHK(pack_norm(e_attn_norm, "encoder.mid.attn_1.norm", bi));
   ECHK(pack_linear(e_qkv, {"encoder.mid.attn_1.q.weight", "encoder.mid.attn_1.k.weight", "encoder.mid.attn_1.v.weight"},
                    {"encoder.mid.attn_1.q.bias", "encoder.mid.attn_1.k.bias", "encoder.mid.attn_1.v.bias"}, bi, bi, PACK_PLAIN));
   ECHK(pack_linear(e_proj, {"encoder.mid.attn_1.proj_out.weight"}, {"encoder.mid.attn_1.proj_out.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(build_vae_res(e_mid2, "encoder.mid.block_2", bi, bi));
+  ECHK(build_res(e_mid2, "encoder.mid.block_2", bi, bi, VAE_RES));
   ECHK(pack_norm(e_norm_out, "encoder.norm_out", bi));
   ECHK(pack_linear(e_conv_out, {"encoder.conv_out.weight"}, {"encoder.conv_out.bias"}, 2 * z, 9 * bi, PACK_CONV3, conv_kpad(bi)));
   ECHK(pack_linear(e_quant, {"quant_conv.weight"}, {"quant_conv.bias"}, 2 * z, 2 * z, PACK_PLAIN));
@@ -1032,7 +981,7 @@ int run_plan(sdxe_engine* e, Plan* p, cudaStream_t stream) {
   ECHK(run_ops(p->pre, stream));
   if (e->profiling) {
     ECHK(run_ops_profiled(e, p->body, stream));
-  } else if (e->use_graph) {
+  } else {
     if (!p->gexec) {
       // capture the body once on a private stream, then replay on the caller's stream
       if (!e->cap_stream) SDXE_CUDA_CHECK(cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking));
@@ -1050,8 +999,6 @@ int run_plan(sdxe_engine* e, Plan* p, cudaStream_t stream) {
       count_launch(p->launches_body);
     }
     SDXE_CUDA_CHECK(cudaGraphLaunch(p->gexec, stream));
-  } else {
-    ECHK(run_ops(p->body, stream));
   }
   ECHK(run_ops(p->post, stream));
   return 0;
@@ -1093,18 +1040,14 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
   Builder B(e, p);
   const bool bf16 = e->bf16;
   const int mc = cfg.model_channels, ted = 4 * mc;
-  const int64_t M0 = (int64_t)n * h * w;
 
   // ---- pre: caller tensors -> plan-owned buffers (outside the graph: caller pointers change per call)
-  const int kin = e->in_blocks[0].conv_in.ld;
-  Buf col0 = e->alloc((size_t)M0 * kin * 2);
   Buf ctx16 = e->alloc((size_t)n * ctx_len * cfg.context_dim * 2);
   Buf temb = e->alloc(sizeof(float) * n * mc);
   Buf y32 = e->alloc(sizeof(float) * std::max(1, n * cfg.adm_in_channels));
   {
-    void* c0 = col0.p; void* cx = ctx16.p; float* te = (float*)temb.p; float* yy = (float*)y32.p;
-    const int cin = cfg.in_channels, cdim = cfg.context_dim, adm = cfg.adm_in_channels;
-    p->pre.push_back([=](cudaStream_t s) { return im2col3x3_nchw_launch(p->x, p->io_dtype, c0, n, cin, h, w, kin, bf16, s); });
+    float* te = (float*)temb.p; float* yy = (float*)y32.p;
+    const int adm = cfg.adm_in_channels;
     p->pre.push_back([=](cudaStream_t s) { return timestep_embedding_launch(p->t, p->io_dtype, te, n, mc, bf16, s); });
     if (adm > 0)
       p->pre.push_back([=](cudaStream_t s) {
@@ -1163,13 +1106,10 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
   for (size_t bi = 0; bi < e->in_blocks.size(); ++bi) {
     const BlockW& b = e->in_blocks[bi];
     if (b.kind == 0) {
-      cur = B.new_act(n, h, w, mc);
-      LinW W = b.conv_in;
-      W.K = W.ld;
-      ECHK(B.gemm(col0.p, W.ld, M0, W, cur.p, Builder::GemmOpt()));
+      ECHK(B.conv_in_nchw(nullptr, n, cfg.in_channels, h, w, b.conv_in, cur));
     } else if (b.kind == 1) {
       Act r;
-      ECHK(B.res_block(b.res, cur, nullptr, emb_ptr, ld_emb, r));
+      ECHK(B.res_block(b.res, cur, nullptr, emb_ptr, ld_emb, 1e-5f, r));
       // `cur` stays alive: it is on the skip stack
       if (b.has_st) {
         Act t;
@@ -1181,8 +1121,7 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
     } else {
       const int Ho = (cur.h + 2 - 3) / 2 + 1, Wo = (cur.w + 2 - 3) / 2 + 1;
       Act d = B.new_act(n, Ho, Wo, b.ch_out);
-      Builder::GemmOpt o;
-      ECHK(B.conv3_s2(cur, b.down, d.p, b.ch_out, o, 1, Ho, Wo));
+      ECHK(B.conv3(cur, b.down, d.p, b.ch_out, Builder::GemmOpt(), 2, 1, Ho, Wo));
       cur = d;
     }
     hs.push_back(cur);
@@ -1190,10 +1129,10 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
   // ---- middle
   {
     Act r1, t, r2;
-    ECHK(B.res_block(e->mid_r1, cur, nullptr, emb_ptr, ld_emb, r1));
+    ECHK(B.res_block(e->mid_r1, cur, nullptr, emb_ptr, ld_emb, 1e-5f, r1));
     ECHK(B.spatial_transformer(e->mid_st, r1, kvbuf.p, e->kv_total, ctx_len, t));
     B.free_act(r1);
-    ECHK(B.res_block(e->mid_r2, t, nullptr, emb_ptr, ld_emb, r2));
+    ECHK(B.res_block(e->mid_r2, t, nullptr, emb_ptr, ld_emb, 1e-5f, r2));
     B.free_act(t);
     cur = r2;  // note: hs.back() (same tensor as the old cur) is still owned by the skip stack
   }
@@ -1205,7 +1144,7 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
     hs.pop_back();
     if (skip.h != cur.h || skip.w != cur.w) EFAIL("unet: skip / hidden size mismatch (latent size must be divisible by 2^(levels-1))");
     Act r;
-    ECHK(B.res_block(b.res, cur, &skip, emb_ptr, ld_emb, r));
+    ECHK(B.res_block(b.res, cur, &skip, emb_ptr, ld_emb, 1e-5f, r));
     if (cur_owned) B.free_act(cur);
     B.free_act(skip);
     if (b.has_st) {
@@ -1215,33 +1154,16 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
       r = t;
     }
     if (b.has_up) {
-      Act up = B.new_act(n, r.h * 2, r.w * 2, r.c);
-      const void* rp = r.p; void* upp = up.p;
-      const int rh = r.h, rw = r.w, rc = r.c;
-      B.ops->push_back([=](cudaStream_t s) { return upsample2x_launch(rp, upp, n, rh, rw, rc, s); });
-      B.free_act(r);
-      Act c = B.new_act(n, up.h, up.w, up.c);
-      ECHK(B.conv3(up, b.up, c.p, up.c, Builder::GemmOpt()));
-      B.free_act(up);
+      Act c;
+      ECHK(B.upsample_conv(r, b.up, c));
       r = c;
     }
     cur = r;
     cur_owned = true;
   }
   // ---- out: GN + SiLU + conv3 -> [M, 8] (4 valid channels)
-  Act g;
-  ECHK(B.group_norm(cur, nullptr, e->out_norm, 1e-5f, true, g));
-  B.free_act(cur);
-  const int ldo = (int)align_up(cfg.out_channels, 8);
-  Buf outb = e->alloc((size_t)M0 * ldo * 2);
-  ECHK(B.conv3(g, e->out_conv, outb.p, ldo, Builder::GemmOpt()));
-  B.free_act(g);
-  {
-    void* ob = outb.p;
-    const int oc = cfg.out_channels, hw = h * w;
-    p->post.push_back([=](cudaStream_t s) { return nhwc_to_nchw_launch(ob, ldo, p->out, p->io_dtype, n, oc, hw, bf16, s); });
-  }
-  // plan-owned buffers (col0, ctx16, temb, y32, e1, emb, l1, emb_all, kvbuf, outb) stay reserved for this plan
+  ECHK(B.out_head(cur, e->out_norm, 1e-5f, e->out_conv));
+  // plan-owned buffers (conv_in's im2col, ctx16, temb, y32, e1, emb, l1, emb_all, kvbuf, out_head's output) stay reserved for this plan
   return 0;
 }
 
@@ -1299,23 +1221,12 @@ int build_vae_encode_plan(sdxe_engine* e, Plan* p, int n, int H, int W) {
   Builder B(e, p);
   const bool bf16 = e->bf16;
   const int nl = cfg.num_levels, cin = cfg.vae_out_ch, z2 = 2 * cfg.vae_z_channels;
-  const int64_t M0 = (int64_t)n * H * W;
-  const int kin = e->e_conv_in.ld;
-  Buf col0 = e->alloc((size_t)M0 * kin * 2);
-  {
-    void* c0 = col0.p;
-    p->pre.push_back([=](cudaStream_t s) { return im2col3x3_nchw_launch(p->x, p->io_dtype, c0, n, cin, H, W, kin, bf16, s); });
-  }
-  Act cur = B.new_act(n, H, W, cfg.vae_ch);
-  {
-    LinW Wc = e->e_conv_in;
-    Wc.K = Wc.ld;
-    ECHK(B.gemm(col0.p, Wc.ld, M0, Wc, cur.p, Builder::GemmOpt()));
-  }
+  Act cur;
+  ECHK(B.conv_in_nchw(nullptr, n, cin, H, W, e->e_conv_in, cur));
   Act t;
   for (int level = 0; level < nl; ++level) {
-    for (const VaeResW& r : e->e_down_blocks[level]) {
-      ECHK(B.vae_res(r, cur, t));
+    for (const ResW& r : e->e_down_blocks[level]) {
+      ECHK(B.res_block(r, cur, nullptr, nullptr, 0, 1e-6f, t));
       B.free_act(cur);
       cur = t;
     }
@@ -1323,16 +1234,16 @@ int build_vae_encode_plan(sdxe_engine* e, Plan* p, int n, int H, int W) {
       // ldm Downsample (with_conv): pad (0,1,0,1) then conv3x3 stride 2, padding 0 -> taps start at the pixel itself
       const int Ho = cur.h / 2, Wo = cur.w / 2;
       Act d = B.new_act(n, Ho, Wo, cur.c);
-      ECHK(B.conv3_s2(cur, e->e_down_conv[level], d.p, cur.c, Builder::GemmOpt(), 0, Ho, Wo));
+      ECHK(B.conv3(cur, e->e_down_conv[level], d.p, cur.c, Builder::GemmOpt(), 2, 0, Ho, Wo));
       B.free_act(cur);
       cur = d;
     }
   }
-  ECHK(B.vae_res(e->e_mid1, cur, t));
+  ECHK(B.res_block(e->e_mid1, cur, nullptr, nullptr, 0, 1e-6f, t));
   B.free_act(cur);
   cur = t;
   ECHK(vae_attn_block(e, B, cur, e->e_attn_norm, e->e_qkv, e->e_proj));
-  ECHK(B.vae_res(e->e_mid2, cur, t));
+  ECHK(B.res_block(e->e_mid2, cur, nullptr, nullptr, 0, 1e-6f, t));
   B.free_act(cur);
   cur = t;
   Act g;
@@ -1359,73 +1270,42 @@ int build_vae_plan(sdxe_engine* e, Plan* p, int n, int h, int w) {
   Builder B(e, p);
   const bool bf16 = e->bf16;
   const int z = cfg.vae_z_channels, nl = cfg.num_levels;
-  const int64_t M0 = (int64_t)n * h * w;
-  Buf zq = e->alloc((size_t)M0 * z * 2);
-  const int kin = e->v_conv_in.ld;
-  Buf col0 = e->alloc((size_t)M0 * kin * 2);
+  Buf zq = e->alloc((size_t)n * h * w * z * 2);
   {
-    void* zp = zq.p; void* c0 = col0.p;
+    void* zp = zq.p;
     const float *pw = e->pq_w, *pb = e->pq_b;
     const int hw = h * w;
-    const int edt = e->dt;
     p->pre.push_back([=](cudaStream_t s) {
       const int64_t total = (int64_t)n * z * hw;
       const int blocks = (int)std::min<int64_t>((total + 255) / 256, 4096);
       if (bf16) post_quant_kernel<true><<<blocks, 256, 0, s>>>(p->x, p->io_dtype, pw, pb, (__nv_bfloat16*)zp, n, z, hw);
       else post_quant_kernel<false><<<blocks, 256, 0, s>>>(p->x, p->io_dtype, pw, pb, (__half*)zp, n, z, hw);
-      count_launch();
-      SDXE_CUDA_CHECK(cudaGetLastError());
+      SDXE_LAUNCH_CHECK();
       return 0;
     });
-    p->pre.push_back([=](cudaStream_t s) { return im2col3x3_nchw_launch(zp, edt, c0, n, z, h, w, kin, bf16, s); });
   }
-  int bi = cfg.vae_ch * cfg.channel_mult[nl - 1];
-  Act cur = B.new_act(n, h, w, bi);
-  {
-    LinW W = e->v_conv_in;
-    W.K = W.ld;
-    ECHK(B.gemm(col0.p, W.ld, M0, W, cur.p, Builder::GemmOpt()));
-  }
+  Act cur;
+  ECHK(B.conv_in_nchw(zq.p, n, z, h, w, e->v_conv_in, cur));
   Act t;
-  ECHK(B.vae_res(e->v_mid1, cur, t));
+  ECHK(B.res_block(e->v_mid1, cur, nullptr, nullptr, 0, 1e-6f, t));
   B.free_act(cur);
   cur = t;
   ECHK(vae_attn_block(e, B, cur, e->v_attn_norm, e->v_qkv, e->v_proj));
-  ECHK(B.vae_res(e->v_mid2, cur, t));
+  ECHK(B.res_block(e->v_mid2, cur, nullptr, nullptr, 0, 1e-6f, t));
   B.free_act(cur);
   cur = t;
   for (int level = nl - 1; level >= 0; --level) {
-    for (const VaeResW& r : e->v_up_blocks[level]) {
-      ECHK(B.vae_res(r, cur, t));
+    for (const ResW& r : e->v_up_blocks[level]) {
+      ECHK(B.res_block(r, cur, nullptr, nullptr, 0, 1e-6f, t));
       B.free_act(cur);
       cur = t;
     }
     if (level != 0) {
-      Act up = B.new_act(n, cur.h * 2, cur.w * 2, cur.c);
-      const void* rp = cur.p; void* upp = up.p;
-      const int rh = cur.h, rw = cur.w, rc = cur.c;
-      B.ops->push_back([=](cudaStream_t s) { return upsample2x_launch(rp, upp, n, rh, rw, rc, s); });
-      B.free_act(cur);
-      Act c = B.new_act(n, up.h, up.w, up.c);
-      ECHK(B.conv3(up, e->v_up_conv[level], c.p, up.c, Builder::GemmOpt()));
-      B.free_act(up);
-      cur = c;
+      ECHK(B.upsample_conv(cur, e->v_up_conv[level], t));
+      cur = t;
     }
   }
-  Act g;
-  ECHK(B.group_norm(cur, nullptr, e->v_norm_out, 1e-6f, true, g));
-  const int Ho = cur.h, Wo = cur.w;
-  B.free_act(cur);
-  const int ldo = (int)align_up(cfg.vae_out_ch, 8);
-  Buf outb = e->alloc((size_t)n * Ho * Wo * ldo * 2);
-  ECHK(B.conv3(g, e->v_conv_out, outb.p, ldo, Builder::GemmOpt()));
-  B.free_act(g);
-  {
-    void* ob = outb.p;
-    const int oc = cfg.vae_out_ch, hw = Ho * Wo;
-    p->post.push_back([=](cudaStream_t s) { return nhwc_to_nchw_launch(ob, ldo, p->out, p->io_dtype, n, oc, hw, bf16, s); });
-  }
-  return 0;
+  return B.out_head(cur, e->v_norm_out, 1e-6f, e->v_conv_out);
 }
 
 }  // namespace
@@ -1453,13 +1333,8 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
     const void *tok = e->c_tok, *pos = e->c_pos;
     const int vocab = cfg.clip_vocab;
     plan->pre.push_back([=](cudaStream_t s) {
-      count_launch();
       ECHK(clip_embed_launch((const int32_t*)plan->x, tok, pos, xp, sp, (int)M, T, C, vocab, b, s));
-      if (plan->n_fix > 0) {
-        count_launch();
-        ECHK(clip_fix_launch(plan->fix_rows, plan->fix_vecs, pos, xp, sp, plan->n_fix, (int)M, T, C, b, s));
-      }
-      return 0;
+      return clip_fix_launch(plan->fix_rows, plan->fix_vecs, pos, xp, sp, plan->n_fix, (int)M, T, C, b, s);
     });
   }
   const float scale = 1.0f / sqrtf((float)d);
@@ -1474,7 +1349,7 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
     {
       const void* qp = qkv.p;
       void* ap = att.p;
-      B.ops->push_back(OpRec([=](cudaStream_t s) { count_launch(); return causal_attn_small_launch(qp, ap, n, T, H, d, scale, b, s); }, K_ATTN,
+      B.ops->push_back(OpRec([=](cudaStream_t s) { return causal_attn_small_launch(qp, ap, n, T, H, d, scale, b, s); }, K_ATTN,
                              2.0 * n * H * (double)T * T * d, 2.0 * (double)M * 4 * C, "causal attn"));
     }
     e->release(qkv);
@@ -1493,7 +1368,7 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
     {
       void* hp = hmid.p;
       const int mode = cfg.clip_act;
-      B.ops->push_back(OpRec([=](cudaStream_t s) { count_launch(); return act_inplace_launch(hp, M * (int64_t)I, mode, b, s); }, K_OTHER, 0.0,
+      B.ops->push_back(OpRec([=](cudaStream_t s) { return act_inplace_launch(hp, M * (int64_t)I, mode, b, s); }, K_OTHER, 0.0,
                              4.0 * (double)M * I, "clip act"));
     }
     Buf x3 = e->alloc((size_t)M * C * 2);
@@ -1512,14 +1387,13 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
     const void* xp = x.p;
     void* yp = y.p;
     const float *g = e->c_final.g, *bt = e->c_final.b;
-    B.ops->push_back(OpRec([=](cudaStream_t s) { count_launch(); return layer_norm_launch(xp, g, bt, yp, (int)M, C, 1e-5f, b, s); }, K_LNORM, 0.0,
+    B.ops->push_back(OpRec([=](cudaStream_t s) { return layer_norm_launch(xp, g, bt, yp, (int)M, C, 1e-5f, b, s); }, K_LNORM, 0.0,
                            4.0 * (double)M * C, "final_layer_norm"));
   }
   {
     const void* yp = y.p;
     const int dt = e->dt;
     plan->post.push_back([=](cudaStream_t s) {
-      count_launch();
       if (plan->io_dtype == SDXE_F32) return cast_to_f32_launch(yp, dt, (float*)plan->out, M * (int64_t)C, false, b, s);
       SDXE_CUDA_CHECK(cudaMemcpyAsync(plan->out, yp, (size_t)M * C * 2, cudaMemcpyDeviceToDevice, s));
       return 0;
@@ -1567,10 +1441,6 @@ Plan* get_plan(sdxe_engine* e, const std::string& key, BuildFn build) {
     it->second->last_use = ++e->tick;
     return it->second.get();
   }
-  static const int env_max = [] { const char* v = getenv("SDXE_MAX_PLANS"); return v ? std::max(1, atoi(v)) : 0; }();
-  static const long env_pool = [] { const char* v = getenv("SDXE_POOL_LIMIT_MB"); return v ? std::max(0l, atol(v)) : -1l; }();
-  if (env_max) e->max_plans = env_max;  // the environment overrides sdxe_set_plan_cache (debugging aid)
-  if (env_pool >= 0) e->pool_limit = (size_t)env_pool << 20;
   while ((int)e->plans.size() >= e->max_plans) evict_lru(e);
   for (int attempt = 0; attempt < 2; ++attempt) {
     std::unique_ptr<Plan> p(new Plan());
@@ -1634,8 +1504,6 @@ int sdxe_create(const sdxe_config* cfg, sdxe_engine** out) {
   e->bf16 = cfg->dtype == SDXE_BF16;
   e->dt = cfg->dtype;
   if (gemm_init() != 0 || attention_init() != 0 || kernels_init() != 0) { delete e; return -1; }
-  const char* ng = getenv("SDXE_NO_GRAPH");
-  e->use_graph = !(ng && ng[0] == '1');
   *out = e;
   return 0;
 }

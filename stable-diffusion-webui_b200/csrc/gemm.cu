@@ -38,7 +38,6 @@ static constexpr int SMEM_BUDGET = 227 * 1024;
 template <int BN, bool BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmArgs a) {
   using T = T16<BF16>;
-  pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t smem_base = (raw + 1023u) & ~1023u;
@@ -66,7 +65,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
     tma_prefetch_desc(&a.tmB);
   }
   __syncthreads();
-  pdl_wait();  // the producing kernel's activations (A, residual) are complete; our output buffer is no longer read
 
   if (warp == CONSUMER_WARPS) {
     // ------------------------------------------------------------------ TMA producer (converged warp, elected issue)
@@ -293,20 +291,14 @@ static size_t gemm_smem_fixed(int num_stages) {  // everything but the operand s
 }
 static size_t gemm_smem(int BN, int num_stages) { return (size_t)num_stages * (A_STAGE_BYTES + BN * 128) + gemm_smem_fixed(num_stages); }
 
-int gemm_pick_stages(int BN) {
+static int gemm_pick_stages(int BN) {
   const int stage_bytes = A_STAGE_BYTES + BN * 128;
   const int s = (int)((SMEM_BUDGET - gemm_smem_fixed(8)) / stage_bytes);
   return std::max(2, std::min(s, 8));
 }
 
-int gemm_finish_args(GemmArgs& a, const void* W, int64_t w_rows, int64_t w_ld) {
-  a.num_stages = gemm_pick_stages(a.BN);
-  if (a.ldo % 8 || (a.residual && a.ldr % 8)) { set_last_error(__FILE__, __LINE__, "gemm: ldo / ldr must be multiples of 8"); return -1; }
-  return make_tmap_2d(&a.tmB, W, w_rows, a.K, w_ld, a.BN);
-}
-
-int gemm_pick_bn(int M, int N, int K, int epi) {
-  (void)K;
+// Tile-width heuristic: pick BN for an [M, N] output (geglu needs BN % 32 == 0 and N % BN == 0).
+static int gemm_pick_bn(int M, int N, int epi) {
   const int sms = num_sms();
   const int num_m = (M + BLOCK_M - 1) / BLOCK_M;
   double best = 1e30;
@@ -323,6 +315,42 @@ int gemm_pick_bn(int M, int N, int K, int epi) {
     if (cost < best - 1e-9) { best = cost; best_bn = bn; }
   }
   return best_bn;
+}
+
+int gemm_args(GemmArgs& a, const GemmA& A, const GemmW& W, void* out, const GemmEpi& o, int bn) {
+  memset(&a, 0, sizeof(a));
+  a.N = W.N; a.K = W.K;
+  if (A.conv) {
+    const int Ho = A.conv == 2 ? A.h / 2 : A.h, Wo = A.conv == 2 ? A.w / 2 : A.w;
+    int bw;
+    if (A.c % 64 || !conv_tile_shape(Ho, Wo, &bw, &a.bh, &a.bn)) { set_last_error(__FILE__, __LINE__, "gemm: conv geometry"); return -1; }
+    a.M = A.n * Ho * Wo; a.K1 = a.K;
+    a.conv = A.conv; a.pad_lo = A.pad_lo; a.cblocks = A.c / 64; a.H = Ho; a.W = Wo;
+    if ((A.conv == 2 ? make_tmap_nhwc_s2 : make_tmap_nhwc)(&a.tmA, A.p, A.n, A.h, A.w, A.c, bw, a.bh, a.bn)) return -1;
+    a.tmA2 = a.tmA;
+  } else {
+    a.M = (int)A.M;
+    a.K1 = A.A2 ? A.K1 : W.K;
+    if (make_tmap_2d(&a.tmA, A.p, A.M, a.K1, A.ld, 128)) return -1;
+    if (A.A2) { if (make_tmap_2d(&a.tmA2, A.A2, A.M, W.K - A.K1, W.K - A.K1, 128)) return -1; }
+    else a.tmA2 = a.tmA;
+  }
+  a.epi = o.epi;
+  a.BN = bn ? bn : gemm_pick_bn(a.M, a.N, o.epi);
+  a.num_stages = gemm_pick_stages(a.BN);
+  a.bias = W.bias;
+  a.rowvec = o.rowvec; a.ldrv = o.ldrv; a.rows_per_sample = std::max(1, o.rows_per_sample);
+  a.residual = o.residual; a.ldr = o.ldr;
+  a.out = out;
+  a.ldo = o.ldo ? o.ldo : (o.epi == EPI_GEGLU ? W.N / 2 : (W.N + 7) / 8 * 8);
+  if (W.c1) {  // a weight with a LayerNorm folded in can only be applied with the row statistics of A
+    if (!o.ln_part || A.A2) { set_last_error(__FILE__, __LINE__, "gemm: folded LayerNorm weight without row statistics"); return -1; }
+    a.c1 = W.c1; a.ln_part = o.ln_part; a.ln_parts = o.ln_parts;
+    a.ln_inv_c = 1.0f / (float)W.K; a.ln_eps = 1e-5f;
+  }
+  if (o.stat_out) a.stat_out = o.stat_out((a.N + a.BN - 1) / a.BN);
+  if (a.ldo % 8 || (a.residual && a.ldr % 8)) { set_last_error(__FILE__, __LINE__, "gemm: ldo / ldr must be multiples of 8"); return -1; }
+  return make_tmap_2d(&a.tmB, W.w, W.rows, a.K, W.ld, a.BN);
 }
 
 typedef void (*GemmKernel)(const GemmArgs);
@@ -357,7 +385,7 @@ int gemm_launch(const GemmArgs& a, bool bf16, cudaStream_t stream) {
     set_last_error(__FILE__, __LINE__, "gemm: unsupported LayerNorm-fold / statistics combination");
     return -1;
   }
-  if (a.num_stages < 2) { set_last_error(__FILE__, __LINE__, "gemm: stages (call gemm_finish_args)"); return -1; }
+  if (a.num_stages < 2) { set_last_error(__FILE__, __LINE__, "gemm: stages (fill the arguments with gemm_args)"); return -1; }
   const size_t smem = gemm_smem(a.BN, a.num_stages);
   if (smem > (size_t)SMEM_BUDGET) { set_last_error(__FILE__, __LINE__, "gemm: shared memory budget"); return -1; }
   const int num_m = (a.M + BLOCK_M - 1) / BLOCK_M, num_n = (a.N + a.BN - 1) / a.BN;
@@ -365,8 +393,9 @@ int gemm_launch(const GemmArgs& a, bool bf16, cudaStream_t stream) {
   if (tiles <= 0) return 0;
   if (gemm_init() != 0) return -1;
   const int grid = std::min(tiles, num_sms());
-  SDXE_CUDA_CHECK(launch_k(gemm_variant(a.BN, bf16), dim3(grid), dim3(GEMM_THREADS), smem, stream, a));
-  SDXE_CUDA_CHECK(cudaGetLastError());
+  const GemmKernel kern = gemm_variant(a.BN, bf16);
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(a);
+  SDXE_LAUNCH_CHECK();
   return 0;
 }
 

@@ -1,6 +1,7 @@
 // Argument block of the wgmma GEMM / implicit-GEMM convolution kernel (gemm.cu).
 #pragma once
 #include "common.cuh"
+#include <functional>
 
 namespace sdxe {
 
@@ -42,15 +43,54 @@ struct alignas(64) GemmArgs {
   float2* stat_out;         // [num_n][M]: part n_blk; null = off. Needs EPI_PLAIN, no rowvec.
 };
 
+// A operand: a row-major matrix [M, K1] with row pitch ld, optionally followed along K by a second contiguous matrix
+// A2 [M, K - K1] (the skip-concat read as two K segments); or an NHWC image [n, h, w, c] read by the implicit 3x3
+// convolution, stride 1 with padding 1, or stride 2 with pad_lo zero rows / columns before the image (output h/2 x w/2).
+struct GemmA {
+  const void* p = nullptr;
+  int64_t M = 0, ld = 0;
+  const void* A2 = nullptr;
+  int K1 = 0;
+  int conv = 0;  // GemmArgs::conv
+  int n = 0, h = 0, w = 0, c = 0, pad_lo = 1;
+  static GemmA matrix(const void* p, int64_t M, int64_t ld, const void* A2 = nullptr, int K1 = 0) {
+    GemmA a;
+    a.p = p; a.M = M; a.ld = ld; a.A2 = A2; a.K1 = K1;
+    return a;
+  }
+  static GemmA nhwc(const void* x, int n, int h, int w, int c, int stride = 1, int pad_lo = 1) {
+    GemmA a;
+    a.p = x; a.conv = stride == 2 ? 2 : 1; a.n = n; a.h = h; a.w = w; a.c = c; a.pad_lo = pad_lo;
+    return a;
+  }
+};
+// Packed weight [rows, ld] 16-bit, K-contiguous; rows >= N (zero rows keep a TMA box inside the tensor). c1: the row sums
+// of a weight with a LayerNorm folded in (then the epilogue needs the row statistics of A).
+struct GemmW {
+  const void* w = nullptr;
+  int64_t rows = 0, ld = 0;
+  int N = 0, K = 0;
+  const float* bias = nullptr;
+  const float* c1 = nullptr;
+};
+struct GemmEpi {
+  int epi = EPI_PLAIN;
+  int ldo = 0;  // 0: N rounded up to 8 (EPI_GEGLU: N / 2)
+  const float* rowvec = nullptr;
+  int ldrv = 0, rows_per_sample = 1;
+  const void* residual = nullptr;
+  int ldr = 0;
+  const float2* ln_part = nullptr;  // statistics of the A rows, for a weight with a folded LayerNorm
+  int ln_parts = 0;
+  // set: emit per-row partial statistics of the output (stat_out) into the [parts][M] buffer this returns, parts = the
+  // number of column tiles of the chosen BN
+  std::function<float2*(int parts)> stat_out;
+};
+// Fills `a` for out = A W^T with epilogue `o`: tensor maps, tile width (bn > 0 forces it), stage count. Returns 0 / -1.
+int gemm_args(GemmArgs& a, const GemmA& A, const GemmW& W, void* out, const GemmEpi& o, int bn = 0);
 // Launch on `stream`. bf16 selects the 16-bit format of A/B/out/residual. Returns 0 / -1.
 int gemm_launch(const GemmArgs& a, bool bf16, cudaStream_t stream);
 int gemm_init();  // one-time kernel attribute setup (call before any stream capture)
-// Tile-width heuristic: pick BN for an [M, N] output (geglu needs BN % 32 == 0 and N % BN == 0).
-int gemm_pick_bn(int M, int N, int K, int epi);
-int gemm_pick_stages(int BN);
-// After M/N/K/K1/BN/epi/tmA/out/ldo/residual/ldr are set: picks the stage count and builds tmB over the packed
-// weights W [w_rows, K] (row pitch w_ld).
-int gemm_finish_args(GemmArgs& a, const void* W, int64_t w_rows, int64_t w_ld);
 // 128-pixel tile of the implicit-GEMM conv as a TMA box (bw x bh x bn); false if (H, W) needs the im2col path.
 bool conv_tile_shape(int H, int W, int* bw, int* bh, int* bn);
 

@@ -1,21 +1,9 @@
 // Bandwidth-bound kernels: GroupNorm / LayerNorm, layout gathers, embeddings, weight repack, sampler-step fusions.
 // All activation tensors are 16-bit NHWC ([n, h*w, c]); vectors of 8 channels (16 B) per thread access.
 #include "kernels.cuh"
-#include <cstdlib>
 #include <algorithm>
-#include <atomic>
 
 namespace sdxe {
-
-static std::atomic<int64_t> g_launches{0};
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
-
-#define SDXE_LAUNCH_CHECK()                 \
-  do {                                      \
-    count_launch();                         \
-    SDXE_CUDA_CHECK(cudaGetLastError());    \
-  } while (0)
 
 SDXE_DEVINL float load_any(const void* p, int dtype, int64_t i) {
   if (dtype == DT_F16) return __half2float(reinterpret_cast<const __half*>(p)[i]);
@@ -55,8 +43,6 @@ SDXE_DEVINL float round16(float v) { return T16<BF16>::to_f(T16<BF16>::from_f(v)
 template <bool BF16>
 __global__ void gn_stats_kernel(const uint4* __restrict__ x1, int c1, const uint4* __restrict__ x2, int c2,
                                 float* __restrict__ partial, int hw, int groups, int pix_per_block) {
-  pdl_launch_dependents();
-  pdl_wait();
   extern __shared__ float sh[];  // [rpi][C] sums, then [rpi][C] sums of squares
   const int C = c1 + c2, V = C >> 3, cpg = C / groups;
   const int n = blockIdx.y;
@@ -94,8 +80,6 @@ __global__ void gn_stats_kernel(const uint4* __restrict__ x1, int c1, const uint
 
 __global__ void gn_finalize_kernel(const float* __restrict__ partial, float* __restrict__ stats, int n_img, int chunks,
                                    int groups, float inv_cnt, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
   // one warp per (image, group): lanes stride over the block partials, fixed-order tree reduce (deterministic)
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= n_img * groups) return;
@@ -127,8 +111,6 @@ __global__ void gn_apply_kernel(const uint4* __restrict__ x1, int c1, const uint
                                 const float* __restrict__ stats, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, uint4* __restrict__ out, int hw, int groups,
                                 int pix_per_block) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int C = c1 + c2, V = C >> 3, cpg = C / groups;
   const int n = blockIdx.y;
   const int vec = threadIdx.x % V, prow = threadIdx.x / V, rpi = blockDim.x / V;
@@ -170,8 +152,6 @@ template <bool BF16, bool SILU>
 __global__ void __launch_bounds__(512) gn_onepass_kernel(const uint32_t* __restrict__ x1, int c1, const uint32_t* __restrict__ x2, int c2,
                                   const float* __restrict__ gamma, const float* __restrict__ beta,
                                   uint32_t* __restrict__ out, int hw, int groups, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
   extern __shared__ uint32_t gn_tile[];  // [hw][W] packed channel pairs
   __shared__ float red[16];
   __shared__ float bcast;
@@ -261,18 +241,14 @@ int group_norm_launch(const void* x1, int c1, const void* x2, int c2, const floa
   if (C % 8 || c1 % 8 || C % groups) { set_last_error(__FILE__, __LINE__, "group_norm: channel alignment"); return -1; }
   if (kernels_init() != 0) return -1;
   {
-    static int onepass = -1;
-    if (onepass < 0) { const char* e = getenv("SDXE_GN_ONEPASS"); onepass = e ? atoi(e) : 1; }
     const int cpg = C / groups;
     const size_t strip = (size_t)hw * cpg * 2;
     // crossover: one CTA per strip wins up to ~48 KB (enough CTAs per SM to hide its serial passes); the
     // wide 64x64 / 32x32 tensors are faster through the three streaming kernels
-    if (onepass && cpg % 2 == 0 && cpg / 2 <= 256 && strip <= 48 * 1024) {
+    if (cpg % 2 == 0 && cpg / 2 <= 256 && strip <= 48 * 1024) {
       const int threads = strip >= 32 * 1024 ? 512 : 256;
       dim3 grid(groups, n);
-#define GN_ONE(B, S)                                                                                                      \
-  SDXE_CUDA_CHECK(launch_k(gn_onepass_kernel<B, S>, grid, dim3(threads), strip, s, (const uint32_t*)x1, c1, (const uint32_t*)x2, c2, \
-                           gamma, beta, (uint32_t*)out, hw, groups, eps))
+#define GN_ONE(B, S) gn_onepass_kernel<B, S><<<grid, threads, strip, s>>>((const uint32_t*)x1, c1, (const uint32_t*)x2, c2, gamma, beta, (uint32_t*)out, hw, groups, eps)
       if (bf16) { if (silu) GN_ONE(true, true); else GN_ONE(true, false); }
       else { if (silu) GN_ONE(false, true); else GN_ONE(false, false); }
 #undef GN_ONE
@@ -294,21 +270,21 @@ int group_norm_launch(const void* x1, int c1, const void* x2, int c2, const floa
   const size_t sm = sizeof(float) * 2 * rpi * C;
   if (kernels_init() != 0) return -1;
   if (bf16)
-    SDXE_CUDA_CHECK(launch_k(gn_stats_kernel<true>, grid, dim3(threads), sm, s, (const uint4*)x1, c1, (const uint4*)x2, c2, partial, hw, groups, ppb));
+    gn_stats_kernel<true><<<grid, threads, sm, s>>>((const uint4*)x1, c1, (const uint4*)x2, c2, partial, hw, groups, ppb);
   else
-    SDXE_CUDA_CHECK(launch_k(gn_stats_kernel<false>, grid, dim3(threads), sm, s, (const uint4*)x1, c1, (const uint4*)x2, c2, partial, hw, groups, ppb));
+    gn_stats_kernel<false><<<grid, threads, sm, s>>>((const uint4*)x1, c1, (const uint4*)x2, c2, partial, hw, groups, ppb);
   SDXE_LAUNCH_CHECK();
   const float inv_cnt = 1.f / ((float)hw * (float)(C / groups));
-  SDXE_CUDA_CHECK(launch_k(gn_finalize_kernel, dim3((n * groups + 3) / 4), dim3(128), 0, s, (const float*)partial, stats, n, chunks, groups, inv_cnt, eps));
+  gn_finalize_kernel<<<(n * groups + 3) / 4, 128, 0, s>>>(partial, stats, n, chunks, groups, inv_cnt, eps);
   SDXE_LAUNCH_CHECK();
   // apply: finer pixel chunks than the statistics pass (pure streaming, wants every SM busy several times over)
   int achunks = std::max(1, std::min((num_sms() * 8 + n - 1) / n, (hw + rpi * 2 - 1) / (rpi * 2)));
   const int appb = (hw + achunks - 1) / achunks;
   achunks = (hw + appb - 1) / appb;
   dim3 agrid(achunks, n);
-#define GN_APPLY(B, S)                                                                                              \
-  SDXE_CUDA_CHECK(launch_k(gn_apply_kernel<B, S>, agrid, dim3(threads), 0, s, (const uint4*)x1, c1, (const uint4*)x2, c2, \
-                           (const float*)stats, gamma, beta, (uint4*)out, hw, groups, appb))
+#define GN_APPLY(B, S)                                                                                                \
+  gn_apply_kernel<B, S><<<agrid, threads, 0, s>>>((const uint4*)x1, c1, (const uint4*)x2, c2, stats, gamma, beta, (uint4*)out, \
+                                                  hw, groups, appb)
   if (bf16) { if (silu) GN_APPLY(true, true); else GN_APPLY(true, false); }
   else { if (silu) GN_APPLY(false, true); else GN_APPLY(false, false); }
 #undef GN_APPLY
@@ -322,8 +298,6 @@ int group_norm_launch(const void* x1, int c1, const void* x2, int c2, const floa
 template <bool BF16, int MAXV>  // MAXV x 32 x 8 channels held in registers (one global read of the row)
 __global__ void __launch_bounds__(256) layer_norm_kernel(const uint4* __restrict__ x, const float* __restrict__ gamma,
                                   const float* __restrict__ beta, uint4* __restrict__ out, int rows, int C, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= rows) return;
   const int V = C >> 3;
@@ -375,8 +349,6 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const uint4* __restrict
 template <bool BF16, int G>
 __global__ void __launch_bounds__(256) layer_norm5_kernel(const uint4* __restrict__ x, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, uint4* __restrict__ out, int rows, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
   constexpr int RPW = 32 / G, V = 5 * G, C = 8 * V;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int row = warp * RPW + lane / G, gl = lane % G;
@@ -428,7 +400,7 @@ int layer_norm_launch(const void* x, const float* gamma, const float* beta, void
   if (c == 320 || c == 640 || c == 1280) {
     const int G = c / 40, rpb = 8 * (32 / G);  // rows per 256-thread block
     const int nb = (rows + rpb - 1) / rpb;
-#define LN5(B, GG) SDXE_CUDA_CHECK(launch_k(layer_norm5_kernel<B, GG>, dim3(nb), dim3(256), 0, s, (const uint4*)x, gamma, beta, (uint4*)out, rows, eps))
+#define LN5(B, GG) layer_norm5_kernel<B, GG><<<nb, 256, 0, s>>>((const uint4*)x, gamma, beta, (uint4*)out, rows, eps)
     if (bf16) { if (G == 8) LN5(true, 8); else if (G == 16) LN5(true, 16); else LN5(true, 32); }
     else { if (G == 8) LN5(false, 8); else if (G == 16) LN5(false, 16); else LN5(false, 32); }
 #undef LN5
@@ -437,7 +409,7 @@ int layer_norm_launch(const void* x, const float* gamma, const float* beta, void
   }
   const int blocks = (rows + 7) / 8;  // 8 warps (rows) per block
   const int nv = (c / 8 + 31) / 32;   // vectors per lane
-#define LN_LAUNCH(B, MV) SDXE_CUDA_CHECK(launch_k(layer_norm_kernel<B, MV>, dim3(blocks), dim3(256), 0, s, (const uint4*)x, gamma, beta, (uint4*)out, rows, c, eps))
+#define LN_LAUNCH(B, MV) layer_norm_kernel<B, MV><<<blocks, 256, 0, s>>>((const uint4*)x, gamma, beta, (uint4*)out, rows, c, eps)
   if (bf16) { if (nv <= 2) LN_LAUNCH(true, 2); else if (nv <= 3) LN_LAUNCH(true, 3); else if (nv <= 5) LN_LAUNCH(true, 5); else LN_LAUNCH(true, 8); }
   else { if (nv <= 2) LN_LAUNCH(false, 2); else if (nv <= 3) LN_LAUNCH(false, 3); else if (nv <= 5) LN_LAUNCH(false, 5); else LN_LAUNCH(false, 8); }
 #undef LN_LAUNCH
@@ -450,8 +422,6 @@ int layer_norm_launch(const void* x, const float* gamma, const float* beta, void
 // =============================================================================================================
 __global__ void im2col3x3_kernel(const uint4* __restrict__ x, uint4* __restrict__ A, int n, int H, int W, int C, int Ho,
                                  int Wo, int stride, int pad_lo, int kpad) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int KV = kpad >> 3;
   const size_t total = (size_t)n * Ho * Wo * KV;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
@@ -477,7 +447,7 @@ int im2col3x3_launch(const void* x, void* A, int n, int H, int W, int C, int Ho,
   if (C % 8 || kpad % 8) { set_last_error(__FILE__, __LINE__, "im2col: alignment"); return -1; }
   const size_t total = (size_t)n * Ho * Wo * (kpad / 8);
   const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
-  SDXE_CUDA_CHECK(launch_k(im2col3x3_kernel, dim3(blocks), dim3(256), 0, s, (const uint4*)x, (uint4*)A, n, H, W, C, Ho, Wo, stride, pad_lo, kpad));
+  im2col3x3_kernel<<<blocks, 256, 0, s>>>((const uint4*)x, (uint4*)A, n, H, W, C, Ho, Wo, stride, pad_lo, kpad);
   SDXE_LAUNCH_CHECK();
   return 0;
 }
@@ -518,8 +488,6 @@ int im2col3x3_nchw_launch(const void* x, int io_dtype, void* A, int n, int C, in
 }
 
 __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int n, int H, int W, int V) {
-  pdl_launch_dependents();
-  pdl_wait();
   const size_t total = (size_t)n * 2 * H * 2 * W * V;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int v = (int)(idx % V);
@@ -535,7 +503,7 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
 int upsample2x_launch(const void* x, void* out, int n, int H, int W, int C, cudaStream_t s) {
   const size_t total = (size_t)n * 4 * H * W * (C / 8);
   const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
-  SDXE_CUDA_CHECK(launch_k(upsample2x_kernel, dim3(blocks), dim3(256), 0, s, (const uint4*)x, (uint4*)out, n, H, W, C / 8));
+  upsample2x_kernel<<<blocks, 256, 0, s>>>((const uint4*)x, (uint4*)out, n, H, W, C / 8);
   SDXE_LAUNCH_CHECK();
   return 0;
 }
@@ -629,8 +597,6 @@ template <bool BF16>
 __global__ void __launch_bounds__(SKL_WARPS * 32)
 skinny_linear_kernel(const float* __restrict__ in, int ldi, const uint4* __restrict__ W, const float* __restrict__ b,
                      const float* add, float* out, int ldo, int M, int N, int K, int silu_out) {
-  pdl_launch_dependents();
-  pdl_wait();
   extern __shared__ __align__(16) uint8_t skl_in[];  // [16][row_bytes] 16-bit activations, K zero-padded to a multiple of 32
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gid = lane >> 2, tig = lane & 3;
@@ -697,9 +663,9 @@ int skinny_linear_launch(const float* in, int ldi, const void* W, const float* b
   if (smem > 200 * 1024) { set_last_error(__FILE__, __LINE__, "skinny_linear: K too large for the activation stage"); return -1; }
   const int blocks = (N + 8 * SKL_WARPS - 1) / (8 * SKL_WARPS);
   if (bf16)
-    SDXE_CUDA_CHECK(launch_k(skinny_linear_kernel<true>, dim3(blocks), dim3(SKL_WARPS * 32), smem, s, in, ldi, (const uint4*)W, b, add, out, ldo, M, N, K, silu_out ? 1 : 0));
+    skinny_linear_kernel<true><<<blocks, SKL_WARPS * 32, smem, s>>>(in, ldi, (const uint4*)W, b, add, out, ldo, M, N, K, silu_out ? 1 : 0);
   else
-    SDXE_CUDA_CHECK(launch_k(skinny_linear_kernel<false>, dim3(blocks), dim3(SKL_WARPS * 32), smem, s, in, ldi, (const uint4*)W, b, add, out, ldo, M, N, K, silu_out ? 1 : 0));
+    skinny_linear_kernel<false><<<blocks, SKL_WARPS * 32, smem, s>>>(in, ldi, (const uint4*)W, b, add, out, ldo, M, N, K, silu_out ? 1 : 0);
   SDXE_LAUNCH_CHECK();
   return 0;
 }

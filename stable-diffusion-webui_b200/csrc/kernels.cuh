@@ -75,7 +75,4 @@ int euler_a_step_launch(float* x, const float* den, const float* noise, float si
 int dpmpp_2m_step_launch(float* x, const float* den, const float* old, float ratio, float neg_expm1, float c0, float c1,
                          int64_t total, cudaStream_t s);
 
-void count_launch(int n = 1);
-int64_t launch_count();
-
 }  // namespace sdxe

@@ -207,7 +207,7 @@ def test_tiny_vae_encoder_geometry(cuda, monkeypatch, tmp_path, dtype, ch_mult, 
 
 
 # ---- stride-2 conv: implicit TMA path vs im2col on the same operands ------------------------------------------------
-# Where conv3_s2 can run implicitly, SDXE_CONV_S2_IMPLICIT=0 sends it through im2col instead. Both feed the GEMM the
+# Where a stride-2 conv3 can run implicitly, SDXE_CONV_S2_IMPLICIT=0 sends it through im2col instead. Both feed the GEMM the
 # same 16-bit operands (TMA's out-of-bounds zero fill is im2col's zero padding, and K runs tap-major, tap * C + c, in
 # both) with the same K = 9C, hence the same tile width and epilogue: the outputs must be bit-identical.
 # The switch is read once per process, so each setting runs in a child process (this file run as a script).
