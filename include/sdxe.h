@@ -132,6 +132,15 @@ int sdxe_clip_forward_fixes(sdxe_engine* e, const int32_t* tokens, void* out, in
  * under the same key skip the cast + GEMM. key = 0 (default) disables the cache. */
 int sdxe_unet_set_context_key(sdxe_engine* e, int64_t key);
 
+/* Hypertile for the next sdxe_unet_forward only (extensions-builtin/hypertile/hypertile.py:269-313): one row
+ * (h', w', nh, nw, max_tiles) of int32 per attn1 (self-attention) layer, in execution order (input blocks, middle block,
+ * output blocks; transformer blocks in order). A row with max_tiles > 0 tiles that layer: its h' * w' tokens, taken as
+ * a row-major h' x w' grid, are regrouped `b (nh h nw w) c -> (b nh nw) (h w) c` and attention runs inside each of the
+ * nh * nw tiles (nh | h', nw | w', nh * nw <= max_tiles). max_tiles = 0 leaves the layer untiled (nh = nw = 1).
+ * The plan is keyed on (h', w', max_tiles) of every row; (nh, nw) change per call without a new plan or graph.
+ * n_layers = 0: no Hypertile (also the state after every forward). */
+int sdxe_unet_set_hypertile(sdxe_engine* e, const int32_t* layers, int n_layers);
+
 /* Execution-plan cache. A plan (buffers from the engine's pool, tensor maps, one CUDA graph) is built per input shape
  * (n, h, w, ctx_len) on first use and replayed afterwards; at most `max_plans` (default 8) are kept, least recently used
  * evicted, and after an eviction free pool memory beyond `pool_limit_mb` (default 6144; < 0 = keep) returns to the
@@ -151,6 +160,12 @@ int sdxe_profile_read(sdxe_engine* e, int kind, double* ms, double* flops, doubl
  * out: [B, Nq, H*D]. D multiple of 8, D <= 512. */
 int sdxe_attention(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int D,
                    float scale, int dtype, void* stream);
+/* Hypertile self-attention of one layer: qkv [B, hp*wp, 3*H*D] (q | k | v, heads contiguous inside each), the tokens a
+ * row-major hp x wp grid cut into nh x nw tiles with (nh, nw) = draw[0], draw[1] (device int32[2], nh | hp, nw | wp,
+ * nh * nw <= max_tiles). qkv_tiled: scratch of qkv's size (the tile-major copy). out: [B, hp*wp, H*D], each token's
+ * attention over the keys of its own tile at the token's own row. */
+int sdxe_hypertile_attention(const void* qkv, void* qkv_tiled, const int32_t* draw, void* out, int B, int H, int hp,
+                             int wp, int D, int max_tiles, float scale, int dtype, void* stream);
 
 /* out[M,N] = A[M,K] W[N,K]^T (+bias[N] fp32) (+residual[M,N]); 16-bit `dtype`; K % 8 == 0, N % 8 == 0.
  * flags: bit0 = GEGLU epilogue (W/bias rows = [value ; gate], out is [M, N/2]). */

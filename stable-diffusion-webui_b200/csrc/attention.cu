@@ -29,7 +29,10 @@ static constexpr int CONSUMER_WARPS = 8;
 static constexpr int KV_BLOCK = 64;
 static constexpr int SMEM_BUDGET = 227 * 1024;
 
-template <bool BF16, int NVS>
+// SEG: Hypertile segmented attention (AttnArgs::seg). A CTA takes query block blockIdx.x % qblocks of tile
+// blockIdx.x / qblocks; CTAs past the drawn tile count exit. Only addressing differs from the plain kernel: a draw of
+// (1, 1) computes bit-identical results.
+template <bool BF16, int NVS, bool SEG>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_constant__ AttnArgs a) {
   using T = T16<BF16>;
   extern __shared__ uint8_t smem_raw[];
@@ -44,10 +47,25 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
   const uint32_t q_full = bar_base + 8u * (2 * NS);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 128;
+  int q0 = blockIdx.x * 128;  // SEG: relative to the tile's first row
+  int Nk = a.Nk;              // SEG: the tile's token count T
+  int row0 = 0;               // SEG: first (tile-major) row of the tile
+  int tile = 0, th = 0, tw = 0, nw = 1;
+  if constexpr (SEG) {
+    const int nh = a.seg[0];
+    nw = a.seg[1];
+    th = a.seg_h / nh;
+    tw = a.seg_w / nw;
+    Nk = th * tw;
+    const int qblocks = (Nk + 127) / 128;
+    tile = blockIdx.x / qblocks;
+    if (tile >= nh * nw) return;  // the grid covers seg_max_tiles tiles
+    row0 = tile * Nk;
+    q0 = (blockIdx.x - tile * qblocks) * 128;
+  }
   const int bh = blockIdx.y;
   const int hb_b = bh / a.H, hb_h = bh - hb_b * a.H;  // (batch, head) coordinates of the 4D per-head tensor maps
-  const int nblk = (a.Nk + KV_BLOCK - 1) / KV_BLOCK;
+  const int nblk = (Nk + KV_BLOCK - 1) / KV_BLOCK;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < NS; ++s) { mbar_init(slot_full(s), 1); mbar_init(slot_empty(s), CONSUMER_WARPS); }
@@ -63,7 +81,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
     // ---------------------------------------------------------------- producer (converged warp, elected issue)
     if (elect_one()) {
       mbar_expect_tx(q_full, a.dqk_slabs * Q_SLAB_BYTES);
-      for (int c = 0; c < a.dqk_slabs; ++c) tma_load_4d(sQ + c * Q_SLAB_BYTES, &a.tmQ, q_full, c * 64, q0, hb_h, hb_b);
+      for (int c = 0; c < a.dqk_slabs; ++c) tma_load_4d(sQ + c * Q_SLAB_BYTES, &a.tmQ, q_full, c * 64, row0 + q0, hb_h, hb_b);
     }
     __syncwarp();
     int slot = 0;
@@ -78,8 +96,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
       if (++slot == NS) { slot = 0; phase ^= 1u; }
     };
     for (int j = 0; j < nblk; ++j) {
-      for (int c = 0; c < a.dqk_slabs; ++c) push(&a.tmK, c * 64, j * KV_BLOCK);
-      for (int vs = 0; vs < NVS; ++vs) push(&a.tmV, vs * 64, j * KV_BLOCK);
+      for (int c = 0; c < a.dqk_slabs; ++c) push(&a.tmK, c * 64, row0 + j * KV_BLOCK);
+      for (int vs = 0; vs < NVS; ++vs) push(&a.tmV, vs * 64, row0 + j * KV_BLOCK);
     }
     return;
   }
@@ -128,12 +146,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
 
     // ---- online softmax on the fragment (a row's 64 columns live in the four threads of a quad)
     const int kv0 = j * KV_BLOCK;
-    if (kv0 + KV_BLOCK > a.Nk) {  // only the last block has invalid key columns
+    if (kv0 + KV_BLOCK > Nk) {  // only the last block has invalid key columns (SEG: keys of the next tile)
 #pragma unroll
       for (int i = 0; i < 8; ++i)
 #pragma unroll
         for (int e = 0; e < 2; ++e)
-          if (kv0 + 8 * i + cq + e >= a.Nk) { s[4 * i + e] = -INFINITY; s[4 * i + 2 + e] = -INFINITY; }
+          if (kv0 + 8 * i + cq + e >= Nk) { s[4 * i + e] = -INFINITY; s[4 * i + 2 + e] = -INFINITY; }
     }
     float mb[2];
 #pragma unroll
@@ -194,8 +212,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv_l = 1.f / l;
-    const int q = q0 + wg * 64 + band + 8 * h;
-    if (q >= a.Nq) continue;
+    int q = q0 + wg * 64 + band + 8 * h;
+    if (q >= (SEG ? Nk : a.Nq)) continue;
+    if constexpr (SEG) {  // tile-major row -> natural row of the seg_h x seg_w grid
+      const int r = q / tw, c = q - r * tw, ih = tile / nw, iw = tile - ih * nw;
+      q = (ih * th + r) * a.seg_w + iw * tw + c;
+    }
     TT* orow = reinterpret_cast<TT*>(a.out) + ((size_t)hb_b * a.Nq + q) * a.ldo + a.out_col0 + hb_h * a.out_hstride;
 #pragma unroll
     for (int vs = 0; vs < NVS; ++vs)
@@ -209,9 +231,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
 }
 
 typedef void (*AttnKernel)(const AttnArgs);
-static AttnKernel attention_variant(bool bf16, int nvs) {
-  if (bf16) return nvs == 1 ? attention_kernel<true, 1> : attention_kernel<true, 2>;
-  return nvs == 1 ? attention_kernel<false, 1> : attention_kernel<false, 2>;
+static AttnKernel attention_variant(bool bf16, int nvs, bool seg) {
+  if (seg) {
+    if (bf16) return nvs == 1 ? attention_kernel<true, 1, true> : attention_kernel<true, 2, true>;
+    return nvs == 1 ? attention_kernel<false, 1, true> : attention_kernel<false, 2, true>;
+  }
+  if (bf16) return nvs == 1 ? attention_kernel<true, 1, false> : attention_kernel<true, 2, false>;
+  return nvs == 1 ? attention_kernel<false, 1, false> : attention_kernel<false, 2, false>;
 }
 
 int attention_init() {
@@ -219,7 +245,9 @@ int attention_init() {
   if (!done) {
     for (int b = 0; b < 2; ++b)
       for (int nvs = 1; nvs <= 2; ++nvs)
-        SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_variant(b != 0, nvs), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET));
+        for (int seg = 0; seg < 2; ++seg)
+          SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_variant(b != 0, nvs, seg != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               SMEM_BUDGET));
     done = true;
   }
   return 0;
@@ -238,9 +266,51 @@ int attention_launch(const AttnArgs& a_in, bool bf16, cudaStream_t stream) {
   if (a.num_slots < std::max(2, a.dqk_slabs)) { set_last_error(__FILE__, __LINE__, "attention: smem"); return -1; }
   const size_t smem = fixed + (size_t)a.num_slots * (SLAB_BYTES + 16);
   if (attention_init() != 0) return -1;
-  dim3 grid((a.Nq + 127) / 128, a.B * a.H);
-  const AttnKernel kern = attention_variant(bf16, a.dv_slabs);
+  const bool seg = a.seg != nullptr;
+  if (seg && (a.Nq != a.Nk || a.seg_h * a.seg_w != a.Nq || a.seg_max_tiles < 1)) {
+    set_last_error(__FILE__, __LINE__, "attention: bad Hypertile geometry");
+    return -1;
+  }
+  // a tiling into k tiles of T tokens needs k ceil(T / 128) <= ceil(Nq / 128) + k - 1 query blocks
+  dim3 grid((a.Nq + 127) / 128 + (seg ? a.seg_max_tiles - 1 : 0), a.B * a.H);
+  const AttnKernel kern = attention_variant(bf16, a.dv_slabs, seg);
   kern<<<grid, ATT_THREADS, smem, stream>>>(a);
+  SDXE_LAUNCH_CHECK();
+  return 0;
+}
+
+__global__ void hypertile_table_kernel(const HtDraws d, int* __restrict__ table) {
+  for (int i = threadIdx.x; i < 2 * d.n; i += blockDim.x) table[i] = d.v[i];
+}
+
+int hypertile_table_launch(const HtDraws& d, int* table, cudaStream_t stream) {
+  if (d.n < 1 || d.n > HT_MAX_LAYERS) { set_last_error(__FILE__, __LINE__, "hypertile: layer count"); return -1; }
+  hypertile_table_kernel<<<1, 256, 0, stream>>>(d, table);
+  SDXE_LAUNCH_CHECK();
+  return 0;
+}
+
+// one CTA per destination row: 16-byte vectors of the row copied from its natural position
+__global__ void hypertile_gather_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int N, int seg_h,
+                                        int seg_w, int row_vecs, const int* __restrict__ seg) {
+  const int nh = seg[0], nw = seg[1];
+  const int th = seg_h / nh, tw = seg_w / nw, T = th * tw;
+  const int64_t p = blockIdx.x;  // b * N + tile-major row
+  const int b = (int)(p / N), l = (int)(p - (int64_t)b * N);
+  const int tile = l / T, t = l - tile * T;
+  const int r = t / tw, c = t - r * tw, ih = tile / nw, iw = tile - ih * nw;
+  const int64_t n = (int64_t)b * N + (int64_t)(ih * th + r) * seg_w + iw * tw + c;
+  const uint4* s = src + n * row_vecs;
+  uint4* o = dst + p * row_vecs;
+  for (int i = threadIdx.x; i < row_vecs; i += blockDim.x) o[i] = s[i];
+}
+
+int hypertile_gather_launch(const void* src, void* dst, int B, int seg_h, int seg_w, int row_elems, const int* seg,
+                            cudaStream_t stream) {
+  if (row_elems % 8 || B < 1 || seg_h < 1 || seg_w < 1) { set_last_error(__FILE__, __LINE__, "hypertile gather: shape"); return -1; }
+  const int row_vecs = row_elems / 8;
+  hypertile_gather_kernel<<<(unsigned)((int64_t)B * seg_h * seg_w), std::min(256, (row_vecs + 31) / 32 * 32), 0, stream>>>(
+      (const uint4*)src, (uint4*)dst, seg_h * seg_w, seg_h, seg_w, row_vecs, seg);
   SDXE_LAUNCH_CHECK();
   return 0;
 }

@@ -22,6 +22,12 @@ struct alignas(64) AttnArgs {
   int ldo;
   int out_col0;
   int out_hstride;
+  // Hypertile (segmented) attention, seg != null: the Nq = Nk tokens of a batch are the tile-major rows of an
+  // seg_h x seg_w grid cut into nh x nw tiles, (nh, nw) = seg[0], seg[1] read from device memory at run time. Each query
+  // attends to the T = (seg_h / nh) (seg_w / nw) keys of its own tile and its output row goes back to its natural
+  // (row-major grid) position. The grid is sized for seg_max_tiles tiles.
+  const int* seg;
+  int seg_h, seg_w, seg_max_tiles;
 };
 
 static constexpr int ATTN_Q_BOX_ROWS = 128;
@@ -40,5 +46,18 @@ int attention_args(std::vector<AttnArgs>& passes, const AttnView& q, const AttnV
                    int Nq, int Nk, int dqk, int dv, float scale, void* out, int ldo, int out_hstride);
 int attention_launch(const AttnArgs& a, bool bf16, cudaStream_t stream);
 int attention_init();
+
+// Hypertile (extensions-builtin/hypertile/hypertile.py:269-313): the per-call tile draws (nh, nw) of n layers, passed
+// by value (kernel parameters are captured at launch) and written to table[2 * layer + {0, 1}].
+static constexpr int HT_MAX_LAYERS = 128;
+struct HtDraws {
+  int n;
+  int v[2 * HT_MAX_LAYERS];
+};
+int hypertile_table_launch(const HtDraws& d, int* table, cudaStream_t stream);
+// dst[b, tile-major row] = src[b, natural row] for the B x (seg_h * seg_w) rows of `row_elems` 16-bit elements (a
+// multiple of 8): the regrouping b (nh h nw w) c -> (b nh nw) (h w) c with (nh, nw) = seg[0], seg[1].
+int hypertile_gather_launch(const void* src, void* dst, int B, int seg_h, int seg_w, int row_elems, const int* seg,
+                            cudaStream_t stream);
 
 }  // namespace sdxe

@@ -33,6 +33,27 @@ int sdxe_attention(const void* q, const void* k, const void* v, void* out, int B
   return 0;
 }
 
+int sdxe_hypertile_attention(const void* qkv, void* qkv_tiled, const int32_t* draw, void* out, int B, int H, int hp,
+                             int wp, int D, int max_tiles, float scale, int dtype, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (!is16(dtype) || D % 8 != 0 || D > 512 || D <= 0 || B < 1 || H < 1 || hp < 1 || wp < 1 || max_tiles < 1 || !draw) {
+    set_last_error(__FILE__, __LINE__, "sdxe_hypertile_attention: bad argument");
+    return -2;
+  }
+  const int N = hp * wp, ld = 3 * H * D;
+  std::vector<AttnArgs> passes;
+  const char* t = (const char*)qkv_tiled;
+  if (attention_args(passes, {t, ld, D, (int64_t)N * ld}, {t + 2 * H * D, ld, D, (int64_t)N * ld},
+                     {t + 4 * H * D, ld, D, (int64_t)N * ld}, B, H, N, N, D, D, scale, out, H * D, D))
+    return -1;
+  if (int rc = hypertile_gather_launch(qkv, qkv_tiled, B, hp, wp, ld, draw, stream)) return rc;
+  for (AttnArgs& a : passes) {
+    a.seg = draw; a.seg_h = hp; a.seg_w = wp; a.seg_max_tiles = max_tiles;
+    if (int rc = attention_launch(a, dtype == SDXE_BF16, stream)) return rc;
+  }
+  return 0;
+}
+
 int sdxe_gemm(const void* A, const void* W, void* out, int M, int N, int K, const float* bias, const void* residual,
               int flags, int dtype, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;

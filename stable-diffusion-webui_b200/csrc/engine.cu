@@ -176,6 +176,8 @@ struct sdxe_engine {
   // same key skips the context cast + projection GEMM (modules/sd_samplers_cfg_denoiser.py re-sends the same cond_in
   // every sampler step).
   int64_t ctx_key = 0;
+  // Hypertile rows (h', w', nh, nw, max_tiles) per attn1 layer for the next sdxe_unet_forward (sdxe_unet_set_hypertile)
+  std::vector<int32_t> ht_rows;
   int max_plans = 8;                    // sdxe_set_plan_cache
   size_t pool_limit = (size_t)6 << 30;  // free (unowned) pool bytes kept after an eviction (sdxe_set_plan_cache)
   uint64_t tick = 0;
@@ -240,6 +242,7 @@ struct Plan {
   int n_fix = 0;
   void* out = nullptr;
   int io_dtype = 0;
+  HtDraws ht_draws{};  // UNet with Hypertile: this call's tile draws, copied into the plan's device table by a pre op
   int launches_body = 0;
   ~Plan() {
     if (gexec) cudaGraphExecDestroy(gexec);
@@ -254,6 +257,11 @@ struct Builder {
   Plan* plan;
   bool bf16;
   std::vector<OpRec>* ops;
+  // Hypertile: rows (h', w', nh, nw, max_tiles) of every attn1 layer in execution order (null: off), the plan's device
+  // table of per-call draws, and the index of the next attn1 layer spatial_transformer emits
+  const std::vector<int32_t>* ht = nullptr;
+  const int* ht_table = nullptr;
+  int ht_next = 0;
 
   Builder(sdxe_engine* e_, Plan* p) : e(e_), plan(p), bf16(e_->bf16), ops(&p->body) {}
 
@@ -376,19 +384,28 @@ struct Builder {
   }
   // q: [B*Nq, ldq], k / v: [B*Nk, ldkv] row-major activations whose columns h*d .. h*d+d-1 belong to head h (the
   // projection GEMM's natural output), seen through per-head views: no padded per-head copy exists.
+  // seg: Hypertile segmented self-attention over the tile-major rows of an seg_h x seg_w grid (AttnArgs::seg); its
+  // FLOP estimate assumes the largest tile count, seg_mt.
   int attention(const void* q, const void* k, const void* v, int B, int H, int Nq, int Nk, int d, int ldq, int ldkv,
-                float scale, void* out, int ldo, int dv_total) {
+                float scale, void* out, int ldo, int dv_total, const int* seg = nullptr, int seg_h = 0, int seg_w = 0,
+                int seg_mt = 0) {
     std::vector<AttnArgs> passes;
     const AttnView vq = {q, ldq, d, (int64_t)Nq * ldq}, vk = {k, ldkv, d, (int64_t)Nk * ldkv}, vv = {v, ldkv, d, (int64_t)Nk * ldkv};
     ECHK(attention_args(passes, vq, vk, vv, B, H, Nq, Nk, d, dv_total, scale, out, ldo, dv_total));
     const int dpad = (d + 63) / 64 * 64;
-    for (const AttnArgs& a : passes) {  // value columns in passes (VAE d = 512, SD1.5 d = 160)
+    for (AttnArgs a : passes) {  // value columns in passes (VAE d = 512, SD1.5 d = 160)
       const int dv = a.dv;
       const bool b = bf16;
-      const double fl = 2.0 * (double)B * H * Nq * Nk * ((double)d + dv);
+      const double keys = seg ? (double)Nk / seg_mt : (double)Nk;
+      const double fl = 2.0 * (double)B * H * Nq * keys * ((double)d + dv);
       const double by = 2.0 * (double)B * H * ((double)Nq * d + (double)Nk * (d + dv) + (double)Nq * dv);
       char dsc[160];
-      snprintf(dsc, sizeof(dsc), "attn B=%d H=%d Nq=%d Nk=%d d=%d dpad=%d dv=%d", B, H, Nq, Nk, d, dpad, dv);
+      if (seg) {
+        a.seg = seg; a.seg_h = seg_h; a.seg_w = seg_w; a.seg_max_tiles = seg_mt;
+        snprintf(dsc, sizeof(dsc), "attn B=%d H=%d Nq=%d Nk=%d d=%d dpad=%d dv=%d ht=%dx%d/%d", B, H, Nq, Nk, d, dpad, dv, seg_h, seg_w, seg_mt);
+      } else {
+        snprintf(dsc, sizeof(dsc), "attn B=%d H=%d Nq=%d Nk=%d d=%d dpad=%d dv=%d", B, H, Nq, Nk, d, dpad, dv);
+      }
       ops->push_back(OpRec([a, b](cudaStream_t s) { return attention_launch(a, b, s); }, K_ATTN, fl, by, dsc));
     }
     return 0;
@@ -509,9 +526,31 @@ struct Builder {
       ECHK(gemm(h.p, C, M, tb.qkv1, qkv.p, oq));  // columns: [q | k | v], heads contiguous inside each
       free_stats(hs);
       Act att = new_act(x.n, x.h, x.w, C);
-      const uint16_t* qkv16 = (const uint16_t*)qkv.p;
-      ECHK(attention(qkv16, qkv16 + C, qkv16 + 2 * C, B, H, tokens, tokens, dh, 3 * C, 3 * C, scale, att.p, C, dh));
-      free_act(qkv);
+      const int li = ht_next++;
+      if (ht && (*ht)[5 * li + 4] > 0) {
+        // Hypertile: q|k|v rows regrouped tile-major, attention inside each tile, outputs stored at their natural rows
+        const int hp = (*ht)[5 * li], wp = (*ht)[5 * li + 1], mt = (*ht)[5 * li + 4];
+        if ((int64_t)hp * wp != tokens) EFAIL("sdxe_unet_set_hypertile: h' * w' differs from the layer's token count");
+        Act qkvt = new_act(x.n, x.h, x.w, 3 * C);
+        {
+          const void* src = qkv.p;
+          void* dst = qkvt.p;
+          const int* seg = ht_table + 2 * li;
+          char d[96];
+          snprintf(d, sizeof(d), "ht_gather M=%lld C=%d grid=%dx%d", (long long)M, 3 * C, hp, wp);
+          ops->push_back(OpRec([=](cudaStream_t s) { return hypertile_gather_launch(src, dst, B, hp, wp, 3 * C, seg, s); }, K_OTHER,
+                               0.0, 4.0 * (double)M * 3 * C, d));
+        }
+        free_act(qkv);
+        const uint16_t* t16 = (const uint16_t*)qkvt.p;
+        ECHK(attention(t16, t16 + C, t16 + 2 * C, B, H, tokens, tokens, dh, 3 * C, 3 * C, scale, att.p, C, dh, ht_table + 2 * li, hp,
+                       wp, mt));
+        free_act(qkvt);
+      } else {
+        const uint16_t* qkv16 = (const uint16_t*)qkv.p;
+        ECHK(attention(qkv16, qkv16 + C, qkv16 + 2 * C, B, H, tokens, tokens, dh, 3 * C, 3 * C, scale, att.p, C, dh));
+        free_act(qkv);
+      }
       Act h2 = new_act(x.n, x.h, x.w, C);
       GemmOpt oo;
       oo.residual = h.p; oo.ldr = C; oo.emit = &hs;
@@ -1035,11 +1074,18 @@ int run_ops_profiled(sdxe_engine* e, std::vector<OpRec>& ops, cudaStream_t s) {
 }
 
 // ---- UNet plan -----------------------------------------------------------------------------------------------
-int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len) {
+int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len, const std::vector<int32_t>* ht) {
   const sdxe_config& cfg = e->cfg;
   Builder B(e, p);
   const bool bf16 = e->bf16;
   const int mc = cfg.model_channels, ted = 4 * mc;
+  if (ht) {  // Hypertile: the draws are data, written per call into a plan-owned table that the tiled layers read
+    Buf table = e->alloc(sizeof(int) * ht->size() / 5 * 2);
+    int* tp = (int*)table.p;
+    p->pre.push_back([=](cudaStream_t s) { return hypertile_table_launch(p->ht_draws, tp, s); });
+    B.ht = ht;
+    B.ht_table = tp;
+  }
 
   // ---- pre: caller tensors -> plan-owned buffers (outside the graph: caller pointers change per call)
   Buf ctx16 = e->alloc((size_t)n * ctx_len * cfg.context_dim * 2);
@@ -1579,9 +1625,32 @@ int sdxe_unet_forward(sdxe_engine* e, const void* x, const void* t, const void* 
   if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_forward: engine is not a finalized UNet");
   if (!x || !t || !ctx || !out || n <= 0 || h <= 0 || w <= 0 || ctx_len <= 0) EFAIL("sdxe_unet_forward: bad argument");
   if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_unet_forward: io dtype");
-  const std::string key = "u:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + ":" + std::to_string(ctx_len);
-  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_unet_plan(e, pl, n, h, w, ctx_len); });
+  std::string key = "u:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + ":" + std::to_string(ctx_len);
+  std::vector<int32_t> ht;
+  ht.swap(e->ht_rows);  // a Hypertile table applies to one call
+  HtDraws draws;
+  if (!ht.empty()) {
+    // the plan is keyed on the structural part (h', w', max_tiles per layer); the draws (nh, nw) are data
+    int n_attn1 = (int)e->mid_st.blocks.size();
+    for (const auto* blocks : {&e->in_blocks, &e->out_blocks})
+      for (const BlockW& b : *blocks)
+        if (b.has_st) n_attn1 += (int)b.st.blocks.size();
+    draws.n = (int)ht.size() / 5;
+    if (draws.n != n_attn1) EFAIL("sdxe_unet_forward: the Hypertile table needs one row per attn1 layer");
+    key += ":ht";
+    for (int i = 0; i < draws.n; ++i) {
+      const int32_t* r = &ht[5 * i];
+      const int hp = r[0], wp = r[1], nh = r[2], nw = r[3], mt = r[4];
+      if (mt > 0 ? (hp < 1 || wp < 1 || nh < 1 || nw < 1 || hp % nh || wp % nw || nh * nw > mt) : (nh != 1 || nw != 1))
+        EFAIL("sdxe_unet_forward: bad Hypertile row (nh | h', nw | w', nh * nw <= max_tiles; untiled rows draw (1, 1))");
+      draws.v[2 * i] = nh;
+      draws.v[2 * i + 1] = nw;
+      key += mt > 0 ? "," + std::to_string(hp) + "x" + std::to_string(wp) + "/" + std::to_string(mt) : ",-";
+    }
+  }
+  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_unet_plan(e, pl, n, h, w, ctx_len, ht.empty() ? nullptr : &ht); });
   if (!p) return -1;
+  if (!ht.empty()) p->ht_draws = draws;
   p->x = x; p->t = t; p->ctx = ctx; p->y = y; p->out = out; p->io_dtype = io_dtype;
   return run_plan(e, p, (cudaStream_t)stream);
 }
@@ -1608,6 +1677,13 @@ int sdxe_clip_forward_fixes(sdxe_engine* e, const int32_t* tokens, void* out, in
 int sdxe_unet_set_context_key(sdxe_engine* e, int64_t key) {
   if (!e || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_set_context_key: not a UNet engine");
   e->ctx_key = key;
+  return 0;
+}
+
+int sdxe_unet_set_hypertile(sdxe_engine* e, const int32_t* layers, int n_layers) {
+  if (!e || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_set_hypertile: not a UNet engine");
+  if (n_layers < 0 || n_layers > HT_MAX_LAYERS || (n_layers > 0 && !layers)) EFAIL("sdxe_unet_set_hypertile: bad argument");
+  e->ht_rows.assign(layers, layers + 5 * n_layers);
   return 0;
 }
 

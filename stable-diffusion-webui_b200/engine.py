@@ -219,10 +219,12 @@ class UNetEngine(_EngineBase):
         super().__init__(cfg, dtype, device)
 
     def forward(self, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor, y: Optional[torch.Tensor] = None,
-                out: Optional[torch.Tensor] = None, context_key: int = 0) -> torch.Tensor:
+                out: Optional[torch.Tensor] = None, context_key: int = 0, hypertile=None) -> torch.Tensor:
         """eps = UNet(x, t, context[, y]); all tensors share x.dtype (fp16 / bf16 / fp32), x is [n,4,h,w] NCHW.
         `context_key` != 0: the caller's promise that `context` has the contents it had the last time this key was
-        used — the cross-attention k | v projections are then reused (sdxe_unet_set_context_key)."""
+        used — the cross-attention k | v projections are then reused (sdxe_unet_set_context_key).
+        `hypertile`: rows (h', w', nh, nw, max_tiles), one per attn1 layer in execution order, tile this call's
+        self-attention (sdxe_unet_set_hypertile); None leaves the call exactly as without Hypertile."""
         if not x.is_cuda:
             raise L.SdxeError("sdxe UNet needs CUDA tensors: there is no CPU fallback")
         dt = x.dtype
@@ -234,6 +236,10 @@ class UNetEngine(_EngineBase):
         if out is None:
             out = torch.empty_like(x)
         L.check(self.lib.sdxe_unet_set_context_key(self._h, int(context_key)), "sdxe_unet_set_context_key")
+        if hypertile is not None:
+            flat = [int(v) for row in hypertile for v in row]
+            L.check(self.lib.sdxe_unet_set_hypertile(self._h, (ctypes.c_int32 * len(flat))(*flat), len(flat) // 5),
+                    "sdxe_unet_set_hypertile")
         L.check(self.lib.sdxe_unet_forward(self._h, L.ptr(x), L.ptr(t), L.ptr(ctx), L.ptr(yy), L.ptr(out), n, h, w,
                                            ctx.shape[1], L.torch_dtype_code(dt), L.current_stream()), "sdxe_unet_forward")
         return out

@@ -70,11 +70,13 @@ SYMBOLS = {
     "sdxe_clip_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "sdxe_clip_forward_fixes": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "sdxe_unet_set_context_key": (c_int, [c_void_p, c_int64]),
+    "sdxe_unet_set_hypertile": (c_int, [c_void_p, POINTER(c_int32), c_int]),
     "sdxe_set_plan_cache": (c_int, [c_void_p, c_int, c_int64]),
     "sdxe_pool_bytes": (c_int64, [c_void_p, POINTER(c_int64)]),
     "sdxe_profile": (c_int, [c_void_p, c_int]),
     "sdxe_profile_read": (c_int, [c_void_p, c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(c_int64)]),
     "sdxe_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
+    "sdxe_hypertile_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
     "sdxe_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "sdxe_conv3x3_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "sdxe_group_norm_nhwc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_void_p]),

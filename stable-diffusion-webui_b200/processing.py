@@ -19,6 +19,7 @@ from typing import List, Optional
 
 import torch
 
+from . import hypertile as HT
 from . import lib as L
 from . import prompt_parser
 from . import samplers as S
@@ -154,6 +155,8 @@ class StableDiffusionProcessingTxt2Img:
     hr_uc: object = None
     step_multiplier: int = 1
     firstpass_steps: int = 0
+    # Hypertile settings of the job (extensions-builtin/hypertile); None: off, no draws
+    hypertile: Optional[HT.HypertileOptions] = None
     # class-level in the reference (shared between jobs so that an unchanged prompt is not re-encoded): [params, result]
     cached_uc = [None, None]
     cached_c = [None, None]
@@ -252,6 +255,8 @@ class StableDiffusionProcessingTxt2Img:
         noise = self.rng.next()
         self.sampler = S.create_sampler(self.sampler_name, self.sd_model)
         self.calculate_hr_conds()                                                  # processing.py:1447 (no-op without prompts)
+        if self.hypertile is not None:                                             # scripts' before_hr (processing.py:1389)
+            self.sd_model.unet.hypertile = HT.begin_hr_pass(self, tw, th)
         c, uc = self.get_conds()
         return self.sampler.sample_img2img(self, samples, noise, c, uc, steps=self.hr_second_pass_steps or self.steps)
 
@@ -348,11 +353,18 @@ def process_images(p: StableDiffusionProcessingTxt2Img, to_host: bool = True) ->
     S.state.interrupted = False
     S.state.skipped = False
     dev = p.sd_model.device
+    unet = p.sd_model.unet
     with torch.cuda.device(dev):
         p.is_hr_pass = False
         p.setup_conds()                                                                       # processing.py:966 (no-op without prompts)
         p.rng = p.make_rng((opt_C, p.height // opt_f, p.width // opt_f), p.seeds)           # processing.py:949
-        samples = p.sample(p.c, p.uc, p.seeds)
+        if p.hypertile is not None:                                                           # scripts' process() (:939)
+            unet.hypertile = HT.begin_job(p)
+        try:
+            samples = p.sample(p.c, p.uc, p.seeds)
+        finally:
+            if p.hypertile is not None:
+                unet.hypertile = None
         if p.do_not_decode:
             return Processed(None, samples, list(p.seeds))
         if p.check_for_nans:  # devices.test_for_nans(samples_ddim, "unet"), processing.py:998 (on unless --disable-nan-check)

@@ -9,6 +9,7 @@ from typing import Dict, Optional
 
 import torch
 
+from . import hypertile as HT
 from . import lib as L
 from .engine import UNetEngine, UNetSpec
 
@@ -17,7 +18,9 @@ try:  # inside the webui process
 
     _SdUnetOptionBase = _ref_sd_unet.SdUnetOption
     _SdUnetBase = _ref_sd_unet.SdUnet
+    IN_WEBUI = True
 except Exception:  # headless: structural twins of modules/sd_unet.py:63-83
+    IN_WEBUI = False
 
     class _SdUnetOptionBase:
         model_name = None
@@ -68,6 +71,10 @@ class SdxeUnet(_SdUnetBase):
         self.dtype = dtype
         self.device_ = torch.device(device)
         self.engine: Optional[UNetEngine] = None
+        # headless Hypertile state of the running job (processing.process_images sets it); in the webui the extension's
+        # hooks on the stock modules are read instead
+        self.hypertile: Optional[HT.HypertileState] = None
+        self._webui_ht_cache = {}
 
     def activate(self):
         if self.engine is not None:
@@ -97,7 +104,23 @@ class SdxeUnet(_SdUnetBase):
         y = kwargs.get("y", args[0] if args else None)
         # context_key: only the package's own CFGDenoiser passes one (it knows the conditioning is step-invariant);
         # called from the stock webui the key is 0 and nothing is cached across calls
-        return self.engine.forward(x, timesteps, context, y, context_key=int(kwargs.get("context_key", 0)))
+        return self.engine.forward(x, timesteps, context, y, context_key=int(kwargs.get("context_key", 0)),
+                                   hypertile=self.hypertile_rows(x.shape[-2], x.shape[-1]))
+
+    def hypertile_rows(self, h: int, w: int):
+        """This call's Hypertile rows (h', w', nh, nw, max_tiles) per attn1 layer, drawn in stock execution order, or None.
+        Every UNet call passes through here, so the draws advance the RNG exactly as the stock hooked modules would."""
+        if IN_WEBUI:
+            try:
+                import hypertile as webui_ht  # extensions-builtin/hypertile/hypertile.py (its RNG_INSTANCE)
+                from modules import shared  # type: ignore
+
+                model = shared.sd_model.model
+            except Exception:  # no Hypertile extension (or no model): nothing is tiled
+                return None
+            st = HT.webui_state(self.engine.spec, model, self._webui_ht_cache)
+            return st.draw_rows(h, w, webui_ht.random_divisor, webui_ht.find_hw_candidates) if st is not None else None
+        return self.hypertile.draw_rows(h, w) if self.hypertile is not None else None
 
 
 class SdxeUnetOption(_SdUnetOptionBase):

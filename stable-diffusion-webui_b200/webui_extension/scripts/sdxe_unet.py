@@ -14,7 +14,10 @@ What the callbacks guard against (a plugin that silently changes results or cras
     the torch modules' weights, which the engine does not read: modules/sd_unet.py:54 moves the stock UNet away);
   * the VAE wrappers are rebuilt whenever model_loaded fires (it also fires after a VAE swap, modules/sd_vae.py:279),
     run in devices.dtype_vae (bf16 when the webui chose it for SDXL; an fp32 VAE — --no-half-vae — is left alone),
-    and anything going wrong restores the stock decode / encode.
+    and anything going wrong restores the stock decode / encode;
+  * Hypertile (extensions-builtin/hypertile): the UNet's tiled self-attention runs on the engine, with the draws taken
+    from the extension's own RNG in stock order (sd_unet.SdxeUnet.hypertile_rows); with Hypertile VAE on, decode and
+    encode go to the stock VAE, which the engine VAE does not tile.
 """
 import os
 import sys
@@ -93,6 +96,10 @@ def _restore_vae(fs):
         eng.close()
 
 
+def _hypertile_vae():
+    return bool(getattr(shared.opts, "hypertile_enable_vae", False))
+
+
 def _model_loaded(sd_model):
     fs = getattr(sd_model, "first_stage_model", None)
     if fs is None:
@@ -110,16 +117,18 @@ def _model_loaded(sd_model):
         engines.append(dec)
         dec.load_state_dict(dsd)
         dec.finalize()
-        fs._sdxe_orig_decode = fs.decode
-        fs.decode = lambda z, *a, **k: dec.decode(z)  # precedent for patching these methods: modules/lowvram.py:64-74,136-137
+        fs._sdxe_orig_decode = orig_decode = fs.decode
+        # precedent for patching these methods: modules/lowvram.py:64-74,136-137. With Hypertile VAE on, the stock
+        # decode runs: its hooks tile the VAE attention and draw from Hypertile's RNG, which the engine VAE does not do
+        fs.decode = lambda z, *a, **k: orig_decode(z, *a, **k) if _hypertile_vae() else dec.decode(z)
         esd = {k: v for k, v in sd.items() if k.startswith(("encoder.", "quant_conv."))}
         if esd:
             enc = VAEEncoderEngine(spec, dtype=dtype, device=shared.device)
             engines.append(enc)
             enc.load_state_dict(esd)
             enc.finalize()
-            fs._sdxe_orig_encode = fs.encode
-            fs.encode = lambda x, *a, **k: _Posterior(enc.encode_moments(x))
+            fs._sdxe_orig_encode = orig_encode = fs.encode
+            fs.encode = lambda x, *a, **k: orig_encode(x, *a, **k) if _hypertile_vae() else _Posterior(enc.encode_moments(x))
         fs._sdxe_engines = engines
     except Exception as ex:  # noqa: BLE001  unknown VAE layout, out of memory, ...: the stock VAE stays in place
         fs._sdxe_engines = engines
