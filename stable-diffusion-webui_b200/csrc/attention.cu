@@ -14,11 +14,13 @@
 //                elements, 8 KB, 128B swizzle) through one in-order ring, in exactly the order they are consumed.
 //   warps 0-7  : two warpgroups of 64 query rows each. S = Q K^T with wgmma from shared memory into registers, online
 //                softmax on the accumulator fragment, P converted in registers into the A operand of O += P V
-//                (V read MN-major straight from its natural [kv, dv] layout), final 1/l scaling and store.
+//                (V read MN-major straight from its natural [kv, dv] layout), final 1/l scaling and store. Each
+//                warpgroup runs the softmax of a block under its O += P V of the previous block.
 #include "attention.cuh"
 #include "wgmma.cuh"
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 
 namespace sdxe {
 
@@ -29,10 +31,28 @@ static constexpr int CONSUMER_WARPS = 8;
 static constexpr int KV_BLOCK = 64;
 static constexpr int SMEM_BUDGET = 227 * 1024;
 
+// One K slab's share of S = Q K^T, committed as one group: the first STEPS k16 steps of the 64-wide slab (acc = 0
+// starts S).
+template <int STEPS, bool BF16> SDXE_DEVINL void qk_slab(float* s, uint64_t qd, uint64_t kd, int acc) {
+  wgmma_fence();
+  wgmma_ss<64, BF16>(s, qd, kd, acc);
+#pragma unroll
+  for (int k = 1; k < STEPS; ++k) wgmma_ss<64, BF16>(s, qd + 2 * k, kd + 2 * k, 1);
+  wgmma_commit();
+}
+// One V slab's O += P V over the 64 keys of a block at width N, committed as one group. V is read MN-major; +16 key
+// rows = +2048 B.
+template <int N, bool BF16> SDXE_DEVINL void pv_slab(float* o, const uint32_t (&pa)[4][4], uint64_t vd) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wgmma_rs_tb<N, BF16>(o, pa[kk], vd + 128 * kk, 1);
+  wgmma_commit();
+}
+
 // SEG: Hypertile segmented attention (AttnArgs::seg). A CTA takes query block blockIdx.x % qblocks of tile
 // blockIdx.x / qblocks; CTAs past the drawn tile count exit. Only addressing differs from the plain kernel: a draw of
 // (1, 1) computes bit-identical results.
-template <bool BF16, int NVS, bool SEG>
+template <bool BF16, int NVS, bool SEG, int HD>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_constant__ AttnArgs a) {
   using T = T16<BF16>;
   extern __shared__ uint8_t smem_raw[];
@@ -95,9 +115,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
       __syncwarp();
       if (++slot == NS) { slot = 0; phase ^= 1u; }
     };
-    for (int j = 0; j < nblk; ++j) {
-      for (int c = 0; c < a.dqk_slabs; ++c) push(&a.tmK, c * 64, row0 + j * KV_BLOCK);
-      for (int vs = 0; vs < NVS; ++vs) push(&a.tmV, vs * 64, row0 + j * KV_BLOCK);
+    // K_0, then K_j before V_{j-1}: the order in which the software-pipelined consumers take them
+    for (int j = 0; j <= nblk; ++j) {
+      if (j < nblk)
+        for (int c = 0; c < a.dqk_slabs; ++c) push(&a.tmK, c * 64, row0 + j * KV_BLOCK);
+      if (j > 0)
+        for (int vs = 0; vs < NVS; ++vs) push(&a.tmV, vs * 64, row0 + (j - 1) * KV_BLOCK);
     }
     return;
   }
@@ -110,6 +133,11 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
   const int cq = 2 * (lane & 3);
   const float sl2 = a.scale_log2;
   const uint64_t qdesc0 = gmma_desc_sw128(sQ + (uint32_t)wg * (64 * 128), 16, 1024);
+  // k16 steps of QK^T in the last K slab and width of O += P V in the last V slab of the pass, for the head dims the
+  // UNets run (d = 40; 80; 160 in passes of 128 and 32 value columns). Steps and columns past the head dim would only
+  // multiply zero padding; any other head dim runs whole 64-wide slabs.
+  constexpr int QK_LAST = HD == 40 ? 3 : HD == 80 ? 1 : HD == 160 ? 2 : 4;
+  constexpr int PV_LAST = HD == 40 ? 40 : HD == 80 ? 16 : (HD == 160 && NVS == 1) ? 32 : 64;
   float o[NVS][32];
 #pragma unroll
   for (int vs = 0; vs < NVS; ++vs)
@@ -123,85 +151,125 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
     if (lane == 0)
       for (int t = 0, s = first; t < count; ++t, s = (s + 1 == NS) ? 0 : s + 1) mbar_arrive(slot_empty(s));
   };
-  mbar_wait(q_full, 0);
 
-  for (int j = 0; j < nblk; ++j) {
-    // ---- S = Q K_j^T
-    float s[32];
-    const int k_first = slot;
-    for (int c = 0; c < a.dqk_slabs; ++c) {
+  // S = Q K_j^T over the next dqk_slabs ring slots, one group per slab
+  auto issue_s = [&](float (&s)[32]) {
+    auto slab = [&](int c, auto steps) {
       mbar_wait(slot_full(slot), phase);
-      wgmma_fence();
       const uint64_t kd = gmma_desc_sw128(sRing + slot * SLAB_BYTES, 16, 1024);
-      const uint64_t qd = qdesc0 + (uint64_t)(c * (Q_SLAB_BYTES >> 4));
+      qk_slab<decltype(steps)::value, BF16>(s, qdesc0 + (uint64_t)(c * (Q_SLAB_BYTES >> 4)), kd, c != 0);
+      advance();
+    };
+    for (int c = 0; c + 1 < a.dqk_slabs; ++c) slab(c, std::integral_constant<int, 4>());
+    slab(a.dqk_slabs - 1, std::integral_constant<int, QK_LAST>());
+  };
+  // O += P V over the next NVS ring slots, one group per slab
+  auto issue_pv = [&](const uint32_t (&pa)[4][4]) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss<64, BF16>(s, qd + 2 * k, kd + 2 * k, (c | k) != 0);
-      wgmma_commit();
+    for (int vs = 0; vs < NVS; ++vs) {
+      mbar_wait(slot_full(slot), phase);
+      const uint64_t vd = gmma_desc_sw128(sRing + slot * SLAB_BYTES, SLAB_BYTES, 1024);
+      if (vs + 1 < NVS) pv_slab<64, BF16>(o[vs], pa, vd);
+      else pv_slab<PV_LAST, BF16>(o[vs], pa, vd);
       advance();
     }
-    wgmma_wait<0>();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) reg_fence(s[i]);
-    release_from(k_first, a.dqk_slabs);
-
-    // ---- online softmax on the fragment (a row's 64 columns live in the four threads of a quad)
-    const int kv0 = j * KV_BLOCK;
-    if (kv0 + KV_BLOCK > Nk) {  // only the last block has invalid key columns (SEG: keys of the next tile)
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 2; ++e)
-          if (kv0 + 8 * i + cq + e >= Nk) { s[4 * i + e] = -INFINITY; s[4 * i + 2 + e] = -INFINITY; }
-    }
+  };
+  // online softmax of block j on the fragment (a row's 64 columns live in the four threads of a quad): updates m and l,
+  // returns the O rescale factor in alpha and the unnormalised probabilities in p. S is only read: ptxas serialises
+  // every wgmma of the kernel if other instructions write accumulator registers while O += P V is in flight (C7515).
+  // MASKED: the block may be the last one, whose key columns past Nk (SEG: keys of the next tile) count as -inf.
+  auto softmax = [&](const float (&s)[32], int j, float (&p)[32], float (&alpha)[2], auto masked) {
+    const int nvalid = Nk - j * KV_BLOCK;
+    auto sv = [&](int r) {  // register r holds column 8 (r / 4) + cq + r % 2
+      return (decltype(masked)::value && 8 * (r >> 2) + cq + (r & 1) >= nvalid) ? -INFINITY : s[r];
+    };
     float mb[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float mx = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(sv(4 * i + 2 * h), sv(4 * i + 2 * h + 1)));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_run[h], mx);  // finite: every block holds at least one valid key
-      const float alpha = ex2_approx((m_run[h] - m_new) * sl2);  // first block: 2^-inf = 0
-      l_run[h] *= alpha;
-#pragma unroll
-      for (int vs = 0; vs < NVS; ++vs)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { o[vs][4 * i + 2 * h] *= alpha; o[vs][4 * i + 2 * h + 1] *= alpha; }
+      alpha[h] = ex2_approx((m_run[h] - m_new) * sl2);  // first block: 2^-inf = 0
+      l_run[h] *= alpha[h];
       m_run[h] = m_new;
       mb[h] = m_new * sl2;
     }
-    // P in the A-operand fragment of m64nNk16: key step kk uses column blocks 2 kk (regs 0, 1) and 2 kk + 1 (regs 2, 3)
-    uint32_t pa[4][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      float p[4];
 #pragma unroll
-      for (int t = 0; t < 4; ++t) p[t] = ex2_approx(fmaf(s[4 * i + t], sl2, -mb[t >> 1]));
-      l_run[0] += p[0] + p[1];
-      l_run[1] += p[2] + p[3];
-      pa[i >> 1][(i & 1) * 2 + 0] = T::pack(p[0], p[1]);
-      pa[i >> 1][(i & 1) * 2 + 1] = T::pack(p[2], p[3]);
+      for (int t = 0; t < 4; ++t) p[4 * i + t] = ex2_approx(fmaf(sv(4 * i + t), sl2, -mb[t >> 1]));
+      l_run[0] += p[4 * i] + p[4 * i + 1];
+      l_run[1] += p[4 * i + 2] + p[4 * i + 3];
     }
-
-    // ---- O += P V_j
-    const int v_first = slot;
+  };
+  // P in the A-operand fragment of m64nNk16: key step kk uses column blocks 2 kk (regs 0, 1) and 2 kk + 1 (regs 2, 3)
+  uint32_t pa[4][4];
+  auto pack_p = [&](const float (&p)[32]) {
 #pragma unroll
-    for (int vs = 0; vs < NVS; ++vs) {
-      mbar_wait(slot_full(slot), phase);
-      wgmma_fence();
-      const uint64_t vd = gmma_desc_sw128(sRing + slot * SLAB_BYTES, SLAB_BYTES, 1024);
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wgmma_rs_tb<64, BF16>(o[vs], pa[kk], vd + 128 * kk, 1);  // +16 key rows = +2048 B
-      wgmma_commit();
-      advance();
+    for (int i = 0; i < 8; ++i) {
+      pa[i >> 1][(i & 1) * 2 + 0] = T::pack(p[4 * i], p[4 * i + 1]);
+      pa[i >> 1][(i & 1) * 2 + 1] = T::pack(p[4 * i + 2], p[4 * i + 3]);
     }
+  };
+  auto wait_o = [&](int v_first) {
     wgmma_wait<0>();
 #pragma unroll
     for (int vs = 0; vs < NVS; ++vs)
 #pragma unroll
       for (int i = 0; i < 32; ++i) reg_fence(o[vs][i]);
     release_from(v_first, NVS);
+  };
+
+  // Software pipeline (per warpgroup): block j's S is waited for, then O += P_{j-1} V_{j-1} is issued and runs on the
+  // tensor cores while the softmax of block j runs. (Issuing S_j and that MMA back to back and waiting for S_j alone
+  // measured slower on H100.) Per row, O, l and m see the same operations in the same order as with no overlap (o = o alpha_j is applied after o += P_{j-1} V_{j-1}, before o += P_j V_j).
+  // The ring holds K_0, K_1, V_0, K_2, V_1, ..., V_{n-1}: consumption order. P_j stays in fp32 until the MMA, which
+  // reads the 16-bit P_{j-1} from registers, is complete.
+  float alpha[2];
+  mbar_wait(q_full, 0);
+  {
+    float s[32], p[32];
+    const int k_first = slot;
+    issue_s(s);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(s[i]);
+    release_from(k_first, a.dqk_slabs);
+    softmax(s, 0, p, alpha, std::true_type());  // alpha = 0 would scale the zero O: nothing to do
+    pack_p(p);
+  }
+  auto step = [&](int j, auto masked) {
+    float s[32], p[32];  // fresh per block, so that only wgmma defines s
+    const int k_first = slot;
+    issue_s(s);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(s[i]);
+    release_from(k_first, a.dqk_slabs);
+    const int v_first = slot;
+    issue_pv(pa);
+    softmax(s, j, p, alpha, masked);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(p[i]);
+    wait_o(v_first);
+    pack_p(p);
+#pragma unroll
+    for (int vs = 0; vs < NVS; ++vs)
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) { o[vs][4 * i + 2 * h] *= alpha[h]; o[vs][4 * i + 2 * h + 1] *= alpha[h]; }
+  };
+  // only the last block can hold keys past Nk: the loop runs the unmasked softmax
+  for (int j = 1; j < nblk - 1; ++j) step(j, std::false_type());
+  if (nblk > 1) step(nblk - 1, std::true_type());
+  {
+    const int v_first = slot;
+    issue_pv(pa);
+    wait_o(v_first);
   }
 
   // ---- epilogue: O / l -> out[b, q, out_col0 + h * out_hstride + j]
@@ -231,13 +299,22 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_kernel(const __grid_
 }
 
 typedef void (*AttnKernel)(const AttnArgs);
-static AttnKernel attention_variant(bool bf16, int nvs, bool seg) {
-  if (seg) {
-    if (bf16) return nvs == 1 ? attention_kernel<true, 1, true> : attention_kernel<true, 2, true>;
-    return nvs == 1 ? attention_kernel<false, 1, true> : attention_kernel<false, 2, true>;
-  }
-  if (bf16) return nvs == 1 ? attention_kernel<true, 1, false> : attention_kernel<true, 2, false>;
-  return nvs == 1 ? attention_kernel<false, 1, false> : attention_kernel<false, 2, false>;
+// head-dim class of a pass (attention_kernel's HD): 40, 80 and 160 for the passes the UNets run, 0 for any other
+static int attention_head_dim(const AttnArgs& a) {
+  if (a.dqk == 40 && a.dv == 40) return 40;
+  if (a.dqk == 80 && a.dv == 80) return 80;
+  if (a.dqk == 160 && (a.dv == 128 || a.dv == 32)) return 160;
+  return 0;
+}
+template <bool BF16, bool SEG> static AttnKernel attention_variant(int nvs, int hd) {
+  if (hd == 40) return attention_kernel<BF16, 1, SEG, 40>;
+  if (hd == 80) return attention_kernel<BF16, 2, SEG, 80>;
+  if (hd == 160) return nvs == 1 ? attention_kernel<BF16, 1, SEG, 160> : attention_kernel<BF16, 2, SEG, 160>;
+  return nvs == 1 ? attention_kernel<BF16, 1, SEG, 0> : attention_kernel<BF16, 2, SEG, 0>;
+}
+static AttnKernel attention_variant(bool bf16, int nvs, bool seg, int hd) {
+  if (seg) return bf16 ? attention_variant<true, true>(nvs, hd) : attention_variant<false, true>(nvs, hd);
+  return bf16 ? attention_variant<true, false>(nvs, hd) : attention_variant<false, false>(nvs, hd);
 }
 
 int attention_init() {
@@ -246,8 +323,9 @@ int attention_init() {
     for (int b = 0; b < 2; ++b)
       for (int nvs = 1; nvs <= 2; ++nvs)
         for (int seg = 0; seg < 2; ++seg)
-          SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_variant(b != 0, nvs, seg != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               SMEM_BUDGET));
+          for (int hd : {0, 40, 80, 160})
+            SDXE_CUDA_CHECK(cudaFuncSetAttribute(attention_variant(b != 0, nvs, seg != 0, hd),
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET));
     done = true;
   }
   return 0;
@@ -273,7 +351,7 @@ int attention_launch(const AttnArgs& a_in, bool bf16, cudaStream_t stream) {
   }
   // a tiling into k tiles of T tokens needs k ceil(T / 128) <= ceil(Nq / 128) + k - 1 query blocks
   dim3 grid((a.Nq + 127) / 128 + (seg ? a.seg_max_tiles - 1 : 0), a.B * a.H);
-  const AttnKernel kern = attention_variant(bf16, a.dv_slabs, seg);
+  const AttnKernel kern = attention_variant(bf16, a.dv_slabs, seg, attention_head_dim(a));
   kern<<<grid, ATT_THREADS, smem, stream>>>(a);
   SDXE_LAUNCH_CHECK();
   return 0;

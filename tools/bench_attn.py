@@ -1,6 +1,7 @@
 """Times the stand-alone attention entry (sdxe_attention) on the UNet's self-attention shapes.
-  python tools/bench_attn.py [--dtype bf16] [--iters 20]
-Prints us / launch, TFLOP/s (4*B*H*Nq*Nk*d) and rel-L2 error vs fp32 SDPA (first shapes only)."""
+  python tools/bench_attn.py [--dtype bf16] [--iters 20] [--dump DIR]
+Prints us / launch, TFLOP/s (4*B*H*Nq*Nk*d) and rel-L2 error vs fp32 SDPA (first shapes only). --dump DIR saves each
+shape's output (seeded inputs) as DIR/<shape>_<dtype>.npy, to compare two builds bit for bit."""
 import argparse
 import os
 import sys
@@ -16,6 +17,7 @@ ap.add_argument("--dtype", default="bf16")
 ap.add_argument("--iters", type=int, default=20)
 ap.add_argument("--shapes", default="sd15_l0,sd15_l1,sd15_l2,sdxl_l1,sdxl_l2,vae64")
 ap.add_argument("--check", action="store_true")
+ap.add_argument("--dump", metavar="DIR", default=None)
 args = ap.parse_args()
 dt = torch.bfloat16 if args.dtype == "bf16" else torch.float16
 SHAPES = {  # B, H, Nq, Nk, d
@@ -48,3 +50,8 @@ for name in args.shapes.split(","):
         ref = ref.transpose(1, 2).reshape(nb, Nq, H * d)
         msg += f"  rel-L2 {((o[:nb].float() - ref).norm() / ref.norm()).item():.3e}"
     print(msg, flush=True)
+    if args.dump:
+        import numpy as np
+
+        os.makedirs(args.dump, exist_ok=True)
+        np.save(os.path.join(args.dump, f"{name}_{args.dtype}.npy"), o.view(torch.int16).cpu().numpy())
