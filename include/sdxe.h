@@ -20,6 +20,9 @@
  *   sdxe_euler_ancestral_step / sdxe_dpmpp_2m_step
  *                       <- k_diffusion/sampling.py sample_euler_ancestral / sample_dpmpp_2m loop bodies
  *                          (called through modules/sd_samplers_kdiffusion.py:230)
+ *   sdxe_set_circular  <- modules/sd_hijack.py:311-318  StableDiffusionModelHijack.apply_circular(enable) (padding_mode
+ *                          'circular' on every Conv2d of the model), driven by the Tiling setting at
+ *                          modules/processing.py:879-880,895
  *   sdxe_create / sdxe_set_weight / sdxe_finalize
  *                       <- modules/sd_unet.py:63-72 SdUnetOption.create_unet() + SdUnet.activate(): the plugin owns
  *                          its weights (the stock UNet is moved to the CPU, modules/sd_unet.py:54)
@@ -140,6 +143,14 @@ int sdxe_unet_set_context_key(sdxe_engine* e, int64_t key);
  * The plan is keyed on (h', w', max_tiles) of every row; (nh, nw) change per call without a new plan or graph.
  * n_layers = 0: no Hypertile (also the state after every forward). */
 int sdxe_unet_set_hypertile(sdxe_engine* e, const int32_t* layers, int n_layers);
+
+/* Tiling (seamless images): with enable != 0, every 3x3 convolution with padding 1 of a UNet, VAE decoder or VAE encoder
+ * engine pads circularly, as torch's padding_mode='circular' (F.pad(x, (1,1,1,1), mode='circular'), then the convolution
+ * without padding): out-of-range taps wrap around the image instead of reading zeros. 1x1 convolutions and the VAE
+ * encoder's stride-2 Downsample (padding 0 after an explicit constant pad) are unchanged. Sticky until changed. The
+ * setting is part of the plan key: enabling builds (once) a plan of its own per shape, disabling returns to the plan
+ * without it. Fails for CLIP engines. */
+int sdxe_set_circular(sdxe_engine* e, int enable);
 
 /* Execution-plan cache. A plan (buffers from the engine's pool, tensor maps, one CUDA graph) is built per input shape
  * (n, h, w, ctx_len) on first use and replayed afterwards; at most `max_plans` (default 8) are kept, least recently used

@@ -178,6 +178,8 @@ struct sdxe_engine {
   int64_t ctx_key = 0;
   // Hypertile rows (h', w', nh, nw, max_tiles) per attn1 layer for the next sdxe_unet_forward (sdxe_unet_set_hypertile)
   std::vector<int32_t> ht_rows;
+  // Circular padding in every 3x3 convolution with padding 1 (sdxe_set_circular): sticky, part of the plan key
+  bool circular = false;
   int max_plans = 8;                    // sdxe_set_plan_cache
   size_t pool_limit = (size_t)6 << 30;  // free (unowned) pool bytes kept after an eviction (sdxe_set_plan_cache)
   uint64_t tick = 0;
@@ -262,8 +264,10 @@ struct Builder {
   const std::vector<int32_t>* ht = nullptr;
   const int* ht_table = nullptr;
   int ht_next = 0;
+  // the plan's 3x3 convolutions with padding wrap around (torch padding_mode='circular') instead of reading zeros
+  bool circular;
 
-  Builder(sdxe_engine* e_, Plan* p) : e(e_), plan(p), bf16(e_->bf16), ops(&p->body) {}
+  Builder(sdxe_engine* e_, Plan* p) : e(e_), plan(p), bf16(e_->bf16), ops(&p->body), circular(e_->circular) {}
 
   Act new_act(int n, int h, int w, int c) {
     Act a;
@@ -321,11 +325,15 @@ struct Builder {
 
   // 3x3 conv of an NHWC activation, W packed [Cout, 9*Cin (ld)]: stride 1 pad 1, or stride 2 (ldm Downsample) with pad_lo
   // zero rows / columns before the image and output Ho x Wo. Implicit GEMM when the geometry allows it, else im2col.
+  // With `circular`, a conv with pad_lo = 1 wraps around instead: im2col indexes modulo H and W, the implicit GEMM reads a
+  // copy of x with its one-pixel circular halo written out (circular_pad_nhwc) with every tap in bounds. pad_lo = 0 (the
+  // VAE encoder's Downsample, Conv2d(padding=0) after a constant pad) keeps its zeros, as padding_mode does not touch it.
   int conv3(const Act& x, const LinW& W, void* out, int ldo, const GemmOpt& o, int stride = 1, int pad_lo = 1, int Ho = 0,
             int Wo = 0) {
     static int s2_implicit = -1;
     if (s2_implicit < 0) { const char* ev = getenv("SDXE_CONV_S2_IMPLICIT"); s2_implicit = ev ? atoi(ev) : 1; }
     if (stride == 1) { Ho = x.h; Wo = x.w; }
+    const bool circ = circular && pad_lo > 0;
     int bw, bh, bn;
     const bool implicit = x.c % 64 == 0 && W.ld == 9 * x.c && conv_tile_shape(Ho, Wo, &bw, &bh, &bn) &&
                           (stride == 1 || (s2_implicit && x.h % 2 == 0 && x.w % 2 == 0 && Ho == x.h / 2 && Wo == x.w / 2));
@@ -337,7 +345,14 @@ struct Builder {
       void* cp = col.p;
       const int n = x.n, H = x.h, Wd = x.w, C = x.c;
       const bool b = bf16;
-      ops->push_back([=](cudaStream_t s) { return im2col3x3_launch(xp, cp, n, H, Wd, C, Ho, Wo, stride, pad_lo, kpad, b, s); });
+      auto fn = [=](cudaStream_t s) { return im2col3x3_launch(xp, cp, n, H, Wd, C, Ho, Wo, stride, pad_lo, kpad, circ, b, s); };
+      if (circ) {
+        char d[160];
+        snprintf(d, sizeof(d), "im2col M=%lld K=%d Cin=%d HxW=%dx%d s=%d circ=1", (long long)M, kpad, C, H, Wd, stride);
+        ops->push_back(OpRec(fn, K_OTHER, 0.0, 2.0 * (double)M * kpad * 2, d));
+      } else {
+        ops->push_back(fn);
+      }
       LinW W2 = W;
       W2.K = kpad;  // zero-padded columns on both sides
       GemmOpt o2 = o;
@@ -349,18 +364,32 @@ struct Builder {
     GemmEpi epi = o;
     epi.ldo = ldo;
     GemmArgs a;
-    ECHK(gemm_args(a, GemmA::nhwc(x.p, x.n, x.h, x.w, x.c, stride, pad_lo), weight(W), out, epi));
     const bool b = bf16;
+    if (circ) {
+      Buf pad = e->alloc((size_t)x.n * (x.h + 2) * (x.w + 2) * x.c * 2);
+      const void* xp = x.p;
+      void* pp = pad.p;
+      const int n = x.n, H = x.h, Wd = x.w, C = x.c;
+      char d[160];
+      snprintf(d, sizeof(d), "circpad n=%d HxW=%dx%d C=%d", n, H, Wd, C);
+      ops->push_back(OpRec([=](cudaStream_t s) { return circular_pad_nhwc_launch(xp, pp, n, H, Wd, C, s); }, K_OTHER, 0.0,
+                           2.0 * n * C * ((double)H * Wd + (double)(H + 2) * (Wd + 2)), d));
+      ECHK(gemm_args(a, GemmA::nhwc(pad.p, n, H + 2, Wd + 2, C, stride, 0, 1), weight(W), out, epi));
+      e->release(pad);  // scratch: the next op that takes it runs after this conv on the same stream
+    } else {
+      ECHK(gemm_args(a, GemmA::nhwc(x.p, x.n, x.h, x.w, x.c, stride, pad_lo), weight(W), out, epi));
+    }
     const double Md = (double)a.M;
     char d[160];
     double by;
     if (stride == 1) {
       by = 2.0 * (Md * x.c + (double)W.N * a.K + Md * W.N + (o.residual ? Md * W.N : 0.0));
-      snprintf(d, sizeof(d), "conv3 M=%d N=%d Cin=%d HxW=%dx%d BN=%d st=%d res=%d rv=%d", a.M, W.N, x.c, x.h, x.w, a.BN, a.num_stages,
-               o.residual ? 1 : 0, o.rowvec ? 1 : 0);
+      snprintf(d, sizeof(d), "conv3 M=%d N=%d Cin=%d HxW=%dx%d BN=%d st=%d res=%d rv=%d%s", a.M, W.N, x.c, x.h, x.w, a.BN, a.num_stages,
+               o.residual ? 1 : 0, o.rowvec ? 1 : 0, circ ? " circ=1" : "");
     } else {
       by = 2.0 * (4.0 * Md * x.c + (double)W.N * a.K + Md * W.N);
-      snprintf(d, sizeof(d), "conv3s2 M=%d N=%d Cin=%d HoxWo=%dx%d BN=%d st=%d", a.M, W.N, x.c, Ho, Wo, a.BN, a.num_stages);
+      snprintf(d, sizeof(d), "conv3s2 M=%d N=%d Cin=%d HoxWo=%dx%d BN=%d st=%d%s", a.M, W.N, x.c, Ho, Wo, a.BN, a.num_stages,
+               circ ? " circ=1" : "");
     }
     ops->push_back(OpRec([a, b](cudaStream_t s) { return gemm_launch(a, b, s); }, K_CONV, 2.0 * Md * W.N * a.K, by, d));
     return 0;
@@ -420,9 +449,9 @@ struct Builder {
       Plan* p = plan;
       void* cp = col.p;
       const int edt = e->dt;
-      const bool b = bf16;
+      const bool b = bf16, circ = circular;
       plan->pre.push_back([=](cudaStream_t s) {
-        return im2col3x3_nchw_launch(src ? src : p->x, src ? edt : p->io_dtype, cp, n, c, h, w, kin, b, s);
+        return im2col3x3_nchw_launch(src ? src : p->x, src ? edt : p->io_dtype, cp, n, c, h, w, kin, circ, b, s);
       });
     }
     out = new_act(n, h, w, W.N);
@@ -1648,6 +1677,7 @@ int sdxe_unet_forward(sdxe_engine* e, const void* x, const void* t, const void* 
       key += mt > 0 ? "," + std::to_string(hp) + "x" + std::to_string(wp) + "/" + std::to_string(mt) : ",-";
     }
   }
+  if (e->circular) key += ":circ";
   Plan* p = get_plan(e, key, [&](Plan* pl) { return build_unet_plan(e, pl, n, h, w, ctx_len, ht.empty() ? nullptr : &ht); });
   if (!p) return -1;
   if (!ht.empty()) p->ht_draws = draws;
@@ -1684,6 +1714,13 @@ int sdxe_unet_set_hypertile(sdxe_engine* e, const int32_t* layers, int n_layers)
   if (!e || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_set_hypertile: not a UNet engine");
   if (n_layers < 0 || n_layers > HT_MAX_LAYERS || (n_layers > 0 && !layers)) EFAIL("sdxe_unet_set_hypertile: bad argument");
   e->ht_rows.assign(layers, layers + 5 * n_layers);
+  return 0;
+}
+
+int sdxe_set_circular(sdxe_engine* e, int enable) {
+  if (!e || (e->cfg.kind != SDXE_MODEL_UNET && e->cfg.kind != SDXE_MODEL_VAE_DECODER && e->cfg.kind != SDXE_MODEL_VAE_ENCODER))
+    EFAIL("sdxe_set_circular: not a UNet or VAE engine");
+  e->circular = enable != 0;
   return 0;
 }
 
@@ -1724,7 +1761,7 @@ int sdxe_vae_decode(sdxe_engine* e, const void* z, void* out, int n, int h, int 
   if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_VAE_DECODER) EFAIL("sdxe_vae_decode: engine is not a finalized VAE decoder");
   if (!z || !out || n <= 0 || h <= 0 || w <= 0) EFAIL("sdxe_vae_decode: bad argument");
   if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_vae_decode: io dtype");
-  const std::string key = "v:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w);
+  const std::string key = "v:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + (e->circular ? ":circ" : "");
   Plan* p = get_plan(e, key, [&](Plan* pl) { return build_vae_plan(e, pl, n, h, w); });
   if (!p) return -1;
   p->x = z; p->out = out; p->io_dtype = io_dtype;
@@ -1736,7 +1773,7 @@ int sdxe_vae_encode(sdxe_engine* e, const void* x, void* out, int n, int h, int 
   const int f = 1 << (e->cfg.num_levels - 1);  // spatial reduction of the encoder (8 for the SD VAE)
   if (!x || !out || n <= 0 || h <= 0 || w <= 0 || (h % f) || (w % f)) EFAIL("sdxe_vae_encode: bad argument (H, W must be multiples of the encoder's downsampling factor)");
   if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_vae_encode: io dtype");
-  const std::string key = "e:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w);
+  const std::string key = "e:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + (e->circular ? ":circ" : "");
   Plan* p = get_plan(e, key, [&](Plan* pl) { return build_vae_encode_plan(e, pl, n, h, w); });
   if (!p) return -1;
   p->x = x; p->out = out; p->io_dtype = io_dtype;

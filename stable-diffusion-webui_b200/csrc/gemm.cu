@@ -13,7 +13,8 @@
 // Structure (one CTA per SM, persistent over output tiles of 128 x BN):
 //   warp 8      : TMA producer. A tile = 128 rows x 64 K (16 KB, 128B swizzle). In conv mode the A tile is a
 //                 4D NHWC box (64 ch x W x bh x bn) fetched at the tap's (dx-1, dy-1) offset: TMA's out-of-bounds
-//                 zero fill IS the convolution padding, so no im2col buffer ever exists.
+//                 zero fill IS the convolution padding, so no im2col buffer ever exists. Circular padding cannot come
+//                 from TMA: there the input carries a materialised one-pixel halo and tap (dy, dx) starts at the pixel.
 //   warps 0-7   : two warpgroups, each owning 64 rows of the tile. wgmma m64nBNk16 straight from the swizzled stages,
 //                 fp32 accumulators in registers (one k-block group in flight while the next is issued), then the
 //                 fused epilogue (bias / LayerNorm fold / timestep-embedding vector / residual / GEGLU / row
@@ -95,7 +96,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
             tma_load_5d(sA, &a.tmA, fb, (tx & 1) * (a.cblocks * BLOCK_K) + cb * BLOCK_K, w0 + (tx >> 1), ty & 1, h0 + (ty >> 1), img0);
           } else if (a.conv) {
             const int dy = tap / 3, dx = tap - dy * 3;
-            tma_load_4d(sA, &a.tmA, fb, cb * BLOCK_K, w0 + dx - 1, h0 + dy - 1, img0);
+            tma_load_4d(sA, &a.tmA, fb, cb * BLOCK_K, w0 + dx - a.pad_lo, h0 + dy - a.pad_lo, img0);
           } else {
             const int k0 = kb * BLOCK_K;
             if (k0 < a.K1) tma_load_2d(sA, &a.tmA, fb, k0, m0);
@@ -321,7 +322,7 @@ int gemm_args(GemmArgs& a, const GemmA& A, const GemmW& W, void* out, const Gemm
   memset(&a, 0, sizeof(a));
   a.N = W.N; a.K = W.K;
   if (A.conv) {
-    const int Ho = A.conv == 2 ? A.h / 2 : A.h, Wo = A.conv == 2 ? A.w / 2 : A.w;
+    const int Ho = (A.h - 2 * A.halo) / A.conv, Wo = (A.w - 2 * A.halo) / A.conv;
     int bw;
     if (A.c % 64 || !conv_tile_shape(Ho, Wo, &bw, &a.bh, &a.bn)) { set_last_error(__FILE__, __LINE__, "gemm: conv geometry"); return -1; }
     a.M = A.n * Ho * Wo; a.K1 = a.K;

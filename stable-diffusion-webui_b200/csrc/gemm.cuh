@@ -18,8 +18,9 @@ struct alignas(64) GemmArgs {
   int K1;            // K elements sourced from tmA (== K when there is no second segment)
   int BN;            // tile width (multiple of 16, <= 256)
   int num_stages;
-  int conv;          // 0 = plain GEMM, 1 = 3x3 stride-1 pad-1 NHWC implicit GEMM, 2 = 3x3 stride-2 (tmA = make_tmap_nhwc_s2)
-  int pad_lo;        // conv == 2: zero rows / columns before the image (1: ldm UNet Downsample, 0: VAE encoder pad (0,1,0,1))
+  int conv;          // 0 = plain GEMM, 1 = 3x3 stride-1 NHWC implicit GEMM, 2 = 3x3 stride-2 (tmA = make_tmap_nhwc_s2)
+  int pad_lo;        // zero rows / columns before the image: 1 (padding 1), or 0: taps start at the pixel (the VAE encoder's
+                     // pad (0,1,0,1) at stride 2; an input that carries its circular halo at either stride)
   int cblocks;       // conv: Cin / 64
   int H, W;          // conv: OUTPUT image size; tile = bn images x bh rows x bw pixels (bw == W, or 128 | W)
   int bh, bn;
@@ -46,21 +47,23 @@ struct alignas(64) GemmArgs {
 // A operand: a row-major matrix [M, K1] with row pitch ld, optionally followed along K by a second contiguous matrix
 // A2 [M, K - K1] (the skip-concat read as two K segments); or an NHWC image [n, h, w, c] read by the implicit 3x3
 // convolution, stride 1 with padding 1, or stride 2 with pad_lo zero rows / columns before the image (output h/2 x w/2).
+// halo = 1: h, w include a one-pixel border already written around the image (circular padding, pad_lo = 0); the output
+// is (h - 2) x (w - 2) at stride 1, (h - 2) / 2 x (w - 2) / 2 at stride 2.
 struct GemmA {
   const void* p = nullptr;
   int64_t M = 0, ld = 0;
   const void* A2 = nullptr;
   int K1 = 0;
   int conv = 0;  // GemmArgs::conv
-  int n = 0, h = 0, w = 0, c = 0, pad_lo = 1;
+  int n = 0, h = 0, w = 0, c = 0, pad_lo = 1, halo = 0;
   static GemmA matrix(const void* p, int64_t M, int64_t ld, const void* A2 = nullptr, int K1 = 0) {
     GemmA a;
     a.p = p; a.M = M; a.ld = ld; a.A2 = A2; a.K1 = K1;
     return a;
   }
-  static GemmA nhwc(const void* x, int n, int h, int w, int c, int stride = 1, int pad_lo = 1) {
+  static GemmA nhwc(const void* x, int n, int h, int w, int c, int stride = 1, int pad_lo = 1, int halo = 0) {
     GemmA a;
-    a.p = x; a.conv = stride == 2 ? 2 : 1; a.n = n; a.h = h; a.w = w; a.c = c; a.pad_lo = pad_lo;
+    a.p = x; a.conv = stride == 2 ? 2 : 1; a.n = n; a.h = h; a.w = w; a.c = c; a.pad_lo = pad_lo; a.halo = halo;
     return a;
   }
 };

@@ -420,8 +420,11 @@ int layer_norm_launch(const void* x, const float* gamma, const float* beta, void
 // =============================================================================================================
 // gathers
 // =============================================================================================================
+// Tap index hi in [-1, H] -> the row circular padding reads (torch padding_mode='circular'); with H = 1 it is row 0 on both sides.
+SDXE_DEVINL int wrap1(int i, int n) { return i < 0 ? i + n : (i >= n ? i - n : i); }
+
 __global__ void im2col3x3_kernel(const uint4* __restrict__ x, uint4* __restrict__ A, int n, int H, int W, int C, int Ho,
-                                 int Wo, int stride, int pad_lo, int kpad) {
+                                 int Wo, int stride, int pad_lo, int kpad, int wrap) {
   const int KV = kpad >> 3;
   const size_t total = (size_t)n * Ho * Wo * KV;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
@@ -435,7 +438,8 @@ __global__ void im2col3x3_kernel(const uint4* __restrict__ x, uint4* __restrict_
       const int ho = (int)((m / Wo) % Ho);
       const int img = (int)(m / ((size_t)Wo * Ho));
       const int dy = tap / 3, dx = tap - dy * 3;
-      const int hi = ho * stride + dy - pad_lo, wi = wo * stride + dx - pad_lo;
+      int hi = ho * stride + dy - pad_lo, wi = wo * stride + dx - pad_lo;
+      if (wrap) { hi = wrap1(hi, H); wi = wrap1(wi, W); }
       if (hi >= 0 && hi < H && wi >= 0 && wi < W) val = __ldg(x + (((size_t)img * H + hi) * W + wi) * (C >> 3) + (c >> 3));
     }
     A[idx] = val;
@@ -443,18 +447,19 @@ __global__ void im2col3x3_kernel(const uint4* __restrict__ x, uint4* __restrict_
 }
 
 int im2col3x3_launch(const void* x, void* A, int n, int H, int W, int C, int Ho, int Wo, int stride, int pad_lo,
-                     int kpad, bool, cudaStream_t s) {
+                     int kpad, bool circular, bool, cudaStream_t s) {
   if (C % 8 || kpad % 8) { set_last_error(__FILE__, __LINE__, "im2col: alignment"); return -1; }
   const size_t total = (size_t)n * Ho * Wo * (kpad / 8);
   const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
-  im2col3x3_kernel<<<blocks, 256, 0, s>>>((const uint4*)x, (uint4*)A, n, H, W, C, Ho, Wo, stride, pad_lo, kpad);
+  im2col3x3_kernel<<<blocks, 256, 0, s>>>((const uint4*)x, (uint4*)A, n, H, W, C, Ho, Wo, stride, pad_lo, kpad,
+                                           circular ? 1 : 0);
   SDXE_LAUNCH_CHECK();
   return 0;
 }
 
 template <bool BF16>
 __global__ void im2col3x3_nchw_kernel(const void* __restrict__ x, int io_dtype, uint4* __restrict__ A, int n, int C,
-                                      int H, int W, int kpad) {
+                                      int H, int W, int kpad, int wrap) {
   const size_t M = (size_t)n * H * W;
   const size_t m = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (m >= M) return;
@@ -468,7 +473,8 @@ __global__ void im2col3x3_nchw_kernel(const void* __restrict__ x, int io_dtype, 
       float val = 0.f;
       if (tap < 9) {
         const int dy = tap / 3, dx = tap - dy * 3;
-        const int hi = h + dy - 1, wi = w + dx - 1;
+        int hi = h + dy - 1, wi = w + dx - 1;
+        if (wrap) { hi = wrap1(hi, H); wi = wrap1(wi, W); }
         if (hi >= 0 && hi < H && wi >= 0 && wi < W) val = load_any(x, io_dtype, (((int64_t)img * C + c) * H + hi) * W + wi);
       }
       v[j] = val;
@@ -477,12 +483,37 @@ __global__ void im2col3x3_nchw_kernel(const void* __restrict__ x, int io_dtype, 
   }
 }
 
-int im2col3x3_nchw_launch(const void* x, int io_dtype, void* A, int n, int C, int H, int W, int kpad, bool bf16,
-                          cudaStream_t s) {
+int im2col3x3_nchw_launch(const void* x, int io_dtype, void* A, int n, int C, int H, int W, int kpad, bool circular,
+                          bool bf16, cudaStream_t s) {
   const size_t M = (size_t)n * H * W;
   const int blocks = (int)((M + 127) / 128);
-  if (bf16) im2col3x3_nchw_kernel<true><<<blocks, 128, 0, s>>>(x, io_dtype, (uint4*)A, n, C, H, W, kpad);
-  else im2col3x3_nchw_kernel<false><<<blocks, 128, 0, s>>>(x, io_dtype, (uint4*)A, n, C, H, W, kpad);
+  const int wrap = circular ? 1 : 0;
+  if (bf16) im2col3x3_nchw_kernel<true><<<blocks, 128, 0, s>>>(x, io_dtype, (uint4*)A, n, C, H, W, kpad, wrap);
+  else im2col3x3_nchw_kernel<false><<<blocks, 128, 0, s>>>(x, io_dtype, (uint4*)A, n, C, H, W, kpad, wrap);
+  SDXE_LAUNCH_CHECK();
+  return 0;
+}
+
+// out[img, i, j] = x[img, (i - 1) mod H, (j - 1) mod W] for i < H + 2, j < W + 2: the one-pixel halo of circular padding
+__global__ void circular_pad_nhwc_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int n, int H, int W, int V) {
+  const int Hp = H + 2, Wp = W + 2;
+  const size_t total = (size_t)n * Hp * Wp * V;
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const int v = (int)(idx % V);
+    size_t p = idx / V;
+    const int wo = (int)(p % Wp);
+    p /= Wp;
+    const int ho = (int)(p % Hp);
+    const int img = (int)(p / Hp);
+    out[idx] = __ldg(x + (((size_t)img * H + wrap1(ho - 1, H)) * W + wrap1(wo - 1, W)) * V + v);
+  }
+}
+
+int circular_pad_nhwc_launch(const void* x, void* out, int n, int H, int W, int C, cudaStream_t s) {
+  if (C % 8) { set_last_error(__FILE__, __LINE__, "circular_pad_nhwc: C % 8"); return -1; }
+  const size_t total = (size_t)n * (H + 2) * (W + 2) * (C / 8);
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
+  circular_pad_nhwc_kernel<<<blocks, 256, 0, s>>>((const uint4*)x, (uint4*)out, n, H, W, C / 8);
   SDXE_LAUNCH_CHECK();
   return 0;
 }

@@ -17,11 +17,15 @@ int layer_norm_launch(const void* x, const float* gamma, const float* beta, void
 
 // ---- layout / gather ---------------------------------------------------------------------------------------
 // 3x3 im2col of NHWC 16-bit input -> A[n*Ho*Wo, kpad], column = tap*C + c, zero padded. pad_lo = top/left padding.
+// circular: taps outside the image wrap around (index mod H, W) instead of reading zero (pad_lo = 1 only).
 int im2col3x3_launch(const void* x, void* A, int n, int H, int W, int C, int Ho, int Wo, int stride, int pad_lo,
-                     int kpad, bool bf16, cudaStream_t s);
-// same, reading an NCHW tensor of `io_dtype` (the UNet / VAE entry convolution on the caller's latent).
-int im2col3x3_nchw_launch(const void* x, int io_dtype, void* A, int n, int C, int H, int W, int kpad, bool bf16,
-                          cudaStream_t s);
+                     int kpad, bool circular, bool bf16, cudaStream_t s);
+// same, stride 1 pad 1, reading an NCHW tensor of `io_dtype` (the UNet / VAE entry convolution on the caller's latent).
+int im2col3x3_nchw_launch(const void* x, int io_dtype, void* A, int n, int C, int H, int W, int kpad, bool circular,
+                          bool bf16, cudaStream_t s);
+// [n, H, W, C] -> [n, H+2, W+2, C] with the wrapped rows, columns and corners of circular padding (C % 8 == 0): the
+// operand of the implicit convolution under circular padding, which then reads every tap in bounds.
+int circular_pad_nhwc_launch(const void* x, void* out, int n, int H, int W, int C, cudaStream_t s);
 int upsample2x_launch(const void* x, void* out, int n, int H, int W, int C, cudaStream_t s);
 // out[n, c, h, w] (io_dtype) = in[(n*hw + p) * ld + c], c < C
 int nhwc_to_nchw_launch(const void* in, int ld, void* out, int io_dtype, int n, int C, int hw, bool bf16, cudaStream_t s);

@@ -158,6 +158,11 @@ class _EngineBase:
     def profile(self, enable: bool):
         L.check(self.lib.sdxe_profile(self._h, 1 if enable else 0), "sdxe_profile")
 
+    def set_circular(self, enable: bool):
+        """Tiling: circular padding in every 3x3 convolution with padding (sdxe_set_circular; UNet and VAE engines, the
+        engine's counterpart of modules/sd_hijack.py:311-318 apply_circular). Sticky until changed."""
+        L.check(self.lib.sdxe_set_circular(self._h, 1 if enable else 0), "sdxe_set_circular")
+
     def set_plan_cache(self, max_plans: int = 8, pool_limit_mb: int = 6144):
         """Bound the per-shape execution-plan cache (LRU) and the free activation pool kept after an eviction."""
         L.check(self.lib.sdxe_set_plan_cache(self._h, int(max_plans), int(pool_limit_mb)), "sdxe_set_plan_cache")

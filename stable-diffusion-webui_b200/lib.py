@@ -71,6 +71,7 @@ SYMBOLS = {
     "sdxe_clip_forward_fixes": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "sdxe_unet_set_context_key": (c_int, [c_void_p, c_int64]),
     "sdxe_unet_set_hypertile": (c_int, [c_void_p, POINTER(c_int32), c_int]),
+    "sdxe_set_circular": (c_int, [c_void_p, c_int]),
     "sdxe_set_plan_cache": (c_int, [c_void_p, c_int, c_int64]),
     "sdxe_pool_bytes": (c_int64, [c_void_p, POINTER(c_int64)]),
     "sdxe_profile": (c_int, [c_void_p, c_int]),

@@ -49,6 +49,7 @@ class SdModel:
         # (FrozenCLIPEmbedderForSDXLWithCustomWords, FrozenOpenCLIPEmbedder2WithCustomWords). None: conds must arrive as tensors.
         self.cond_stage_model = None
         self.sdxl_crop_top, self.sdxl_crop_left = 0, 0   # opts.sdxl_crop_top / sdxl_crop_left
+        self.circular_enabled = False                       # model_hijack.circular_enabled (apply_circular)
 
     def get_learned_conditioning(self, texts):
         """LatentDiffusion.get_learned_conditioning (`cond_stage_model(texts)`); SDXL: modules/sd_models_xl.py:12-34 — width /
@@ -78,6 +79,18 @@ class SdModel:
         if vector is not None:
             kwargs["y"] = vector.to(dt)
         return self.unet.forward(x_in, t.to(dt), context.to(dt), **kwargs)
+
+    def apply_circular(self, enable: bool):
+        """StableDiffusionModelHijack.apply_circular (modules/sd_hijack.py:311-318): Tiling — circular padding in every
+        padded convolution of the UNet, the VAE decoder and the VAE encoder. A repeated identical call does nothing."""
+        enable = bool(enable)
+        if self.circular_enabled == enable:
+            return
+        self.circular_enabled = enable
+        self.unet.set_circular(enable)
+        for eng in (self.vae, self.vae_encoder):
+            if eng is not None:
+                eng.set_circular(enable)
 
     def decode_first_stage(self, z):
         """z already divided by scale_factor upstream? No: the reference's decode_first_stage divides
@@ -157,6 +170,8 @@ class StableDiffusionProcessingTxt2Img:
     firstpass_steps: int = 0
     # Hypertile settings of the job (extensions-builtin/hypertile); None: off, no draws
     hypertile: Optional[HT.HypertileOptions] = None
+    # Tiling (opts.tiling, modules/shared_options.py:184): None takes the option's default, False
+    tiling: Optional[bool] = None
     # class-level in the reference (shared between jobs so that an unchanged prompt is not re-encoded): [params, result]
     cached_uc = [None, None]
     cached_c = [None, None]
@@ -356,6 +371,9 @@ def process_images(p: StableDiffusionProcessingTxt2Img, to_host: bool = True) ->
     unet = p.sd_model.unet
     with torch.cuda.device(dev):
         p.is_hr_pass = False
+        if p.tiling is None:                                                                  # processing.py:879-880
+            p.tiling = False
+        p.sd_model.apply_circular(p.tiling)                                                   # :895
         p.setup_conds()                                                                       # processing.py:966 (no-op without prompts)
         p.rng = p.make_rng((opt_C, p.height // opt_f, p.width // opt_f), p.seeds)           # processing.py:949
         if p.hypertile is not None:                                                           # scripts' process() (:939)

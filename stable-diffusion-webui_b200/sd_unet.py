@@ -40,6 +40,18 @@ except Exception:  # headless: structural twins of modules/sd_unet.py:63-83
             pass
 
 
+def webui_circular() -> bool:
+    """The webui's Tiling state: modules.sd_hijack.model_hijack.circular_enabled, which apply_circular sets
+    (modules/sd_hijack.py:311-318, from modules/processing.py:895). Unreadable means off, as in a webui where
+    apply_circular never ran."""
+    try:
+        from modules import sd_hijack  # type: ignore
+
+        return bool(sd_hijack.model_hijack.circular_enabled)
+    except Exception:
+        return False
+
+
 def guess_unet_spec(state_dict: Dict[str, torch.Tensor]) -> UNetSpec:
     """Architecture from the checkpoint's own keys (the webui guesses from keys too: sd_models_config.py:72-114)."""
     if "label_emb.0.0.weight" in state_dict:
@@ -75,6 +87,8 @@ class SdxeUnet(_SdUnetBase):
         # hooks on the stock modules are read instead
         self.hypertile: Optional[HT.HypertileState] = None
         self._webui_ht_cache = {}
+        # headless Tiling state (SdModel.apply_circular); in the webui model_hijack.circular_enabled is read per call
+        self.circular = False
 
     def activate(self):
         if self.engine is not None:
@@ -88,8 +102,15 @@ class SdxeUnet(_SdUnetBase):
         eng = UNetEngine(spec, dtype=self.dtype, device=self.device_)
         eng.load_state_dict(sd)
         eng.finalize()
+        eng.set_circular(self.circular)
         self.engine = eng
         self._sd = None  # the engine holds the packed copy
+
+    def set_circular(self, enable: bool):
+        """Tiling on the engine (sdxe_set_circular), kept across deactivate() / activate()."""
+        self.circular = bool(enable)
+        if self.engine is not None:
+            self.engine.set_circular(self.circular)
 
     def deactivate(self):
         if self.engine is not None:
@@ -102,6 +123,10 @@ class SdxeUnet(_SdUnetBase):
         if self.engine is None:
             raise L.SdxeError("SdxeUnet.forward before activate()")
         y = kwargs.get("y", args[0] if args else None)
+        if IN_WEBUI:  # the stock convs whose padding_mode apply_circular flipped never run: carry the flag to the engine
+            circular = webui_circular()
+            if circular != self.circular:
+                self.set_circular(circular)
         # context_key: only the package's own CFGDenoiser passes one (it knows the conditioning is step-invariant);
         # called from the stock webui the key is 0 and nothing is cached across calls
         return self.engine.forward(x, timesteps, context, y, context_key=int(kwargs.get("context_key", 0)),

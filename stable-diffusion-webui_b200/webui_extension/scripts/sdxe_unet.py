@@ -17,7 +17,10 @@ What the callbacks guard against (a plugin that silently changes results or cras
     and anything going wrong restores the stock decode / encode;
   * Hypertile (extensions-builtin/hypertile): the UNet's tiled self-attention runs on the engine, with the draws taken
     from the extension's own RNG in stock order (sd_unet.SdxeUnet.hypertile_rows); with Hypertile VAE on, decode and
-    encode go to the stock VAE, which the engine VAE does not tile.
+    encode go to the stock VAE, which the engine VAE does not tile;
+  * Tiling (modules/sd_hijack.py:311-318 apply_circular flips padding_mode on the stock Conv2d modules, which the engine
+    never runs): the UNet and both VAE wrappers read model_hijack.circular_enabled on every call and set it on their
+    engine (sd_unet.webui_circular; unreadable = off). With Hypertile VAE on, the stock VAE's flipped modules do it.
 """
 import os
 import sys
@@ -34,7 +37,7 @@ import torch  # noqa: E402
 from sdwebui_b200.engine import VAEDecoderEngine, VAEEncoderEngine, VAESpec  # noqa: E402
 from sdwebui_b200.lib import SdxeError  # noqa: E402
 from sdwebui_b200.sd_hijack_optimizations import SdOptimizationSdxe  # noqa: E402
-from sdwebui_b200.sd_unet import SdxeUnetOption, guess_unet_spec  # noqa: E402
+from sdwebui_b200.sd_unet import SdxeUnetOption, guess_unet_spec, webui_circular  # noqa: E402
 
 
 def supported_unet_spec(sd_model):
@@ -100,6 +103,12 @@ def _hypertile_vae():
     return bool(getattr(shared.opts, "hypertile_enable_vae", False))
 
 
+def _tiled(eng):
+    """`eng` with the webui's current Tiling state applied (apply_circular may have changed it since the last call)."""
+    eng.set_circular(webui_circular())
+    return eng
+
+
 def _model_loaded(sd_model):
     fs = getattr(sd_model, "first_stage_model", None)
     if fs is None:
@@ -120,7 +129,7 @@ def _model_loaded(sd_model):
         fs._sdxe_orig_decode = orig_decode = fs.decode
         # precedent for patching these methods: modules/lowvram.py:64-74,136-137. With Hypertile VAE on, the stock
         # decode runs: its hooks tile the VAE attention and draw from Hypertile's RNG, which the engine VAE does not do
-        fs.decode = lambda z, *a, **k: orig_decode(z, *a, **k) if _hypertile_vae() else dec.decode(z)
+        fs.decode = lambda z, *a, **k: orig_decode(z, *a, **k) if _hypertile_vae() else _tiled(dec).decode(z)
         esd = {k: v for k, v in sd.items() if k.startswith(("encoder.", "quant_conv."))}
         if esd:
             enc = VAEEncoderEngine(spec, dtype=dtype, device=shared.device)
@@ -128,7 +137,7 @@ def _model_loaded(sd_model):
             enc.load_state_dict(esd)
             enc.finalize()
             fs._sdxe_orig_encode = orig_encode = fs.encode
-            fs.encode = lambda x, *a, **k: orig_encode(x, *a, **k) if _hypertile_vae() else _Posterior(enc.encode_moments(x))
+            fs.encode = lambda x, *a, **k: orig_encode(x, *a, **k) if _hypertile_vae() else _Posterior(_tiled(enc).encode_moments(x))
         fs._sdxe_engines = engines
     except Exception as ex:  # noqa: BLE001  unknown VAE layout, out of memory, ...: the stock VAE stays in place
         fs._sdxe_engines = engines
