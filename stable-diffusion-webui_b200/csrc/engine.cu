@@ -43,10 +43,9 @@ struct RawWeight {
   int dtype = 0;
   std::vector<int64_t> shape;
   int64_t numel = 0;
-  bool used = false;
 };
 
-// ---- packed weights ------------------------------------------------------------------------------------------
+// ---- packed weights ---------------------------------------------------------------------------------------------
 struct LinW {  // 16-bit [N, ld] K-contiguous (+ fp32 bias)
   void* w = nullptr;
   float* b = nullptr;
@@ -84,20 +83,74 @@ struct STW {
   std::vector<TBlockW> blocks;
   int C = 0, heads = 0, dh = 0;
 };
-struct BlockW {  // one TimestepEmbedSequential
-  int kind = 0;  // 0 conv_in, 1 res(+st)(+up), 2 downsample
+
+// ---- UNet (ldm / sgm UNetModel) ---------------------------------------------------------------------------------
+struct UNetBlockW {  // one TimestepEmbedSequential: ResBlock (+ SpatialTransformer) (+ Upsample, output blocks only)
   ResW res;
   bool has_st = false;
   STW st;
   bool has_up = false;
-  LinW up;    // Upsample.conv
+  LinW up;  // Upsample.conv
+};
+struct UNetLevelW {  // the input blocks of one level: its ResBlocks, then a Downsample except at the deepest level
+  std::vector<UNetBlockW> blocks;
+  bool has_down = false;
   LinW down;  // Downsample.op
+};
+struct UNetW {
+  LinW te0, te2, le0, le2, emb_all;
+  int emb_total = 0;
+  // every transformer block's attn2.to_k / to_v stacked along N: the context is projected ONCE per UNet call
+  LinW kv_all;
+  int kv_total = 0;
+  int n_attn1 = 0;  // self-attention layers (one Hypertile row each)
   LinW conv_in;
-  int ch_out = 0;
+  std::vector<UNetLevelW> in_levels;
+  ResW mid_r1, mid_r2;
+  STW mid_st;
+  std::vector<UNetBlockW> out_blocks;
+  NormW out_norm;
+  LinW out_conv;
+  // Cross-attention K / V cache: a non-zero key is the caller's promise that the context passed under that key always has
+  // the same contents (the conditioning of one job is step-invariant); a plan whose k|v buffer was last filled under the
+  // same key skips the context cast + projection GEMM (modules/sd_samplers_cfg_denoiser.py re-sends the same cond_in
+  // every sampler step).
+  int64_t ctx_key = 0;
+  // Hypertile rows (h', w', nh, nw, max_tiles) per attn1 layer for the next sdxe_unet_forward (sdxe_unet_set_hypertile)
+  std::vector<int32_t> ht_rows;
 };
 
+// ---- VAE (ldm Encoder / Decoder of AutoencoderKL) ---------------------------------------------------------------
+struct VaeMidW {  // mid: ResBlock -> AttnBlock (GN -> q|k|v -> single-head attention -> proj_out + x) -> ResBlock
+  ResW r1, r2;
+  NormW attn_norm;
+  LinW qkv, proj;
+};
+struct VaeLevelW {  // down.{l} / up.{l}: ResBlocks, then the level's Downsample / Upsample conv if it has one
+  std::vector<ResW> blocks;
+  bool has_resample = false;
+  LinW resample;
+};
+struct VaeW {
+  LinW conv_in;
+  std::vector<VaeLevelW> levels;  // level index as in the state dict
+  VaeMidW mid;
+  NormW norm_out;
+  LinW conv_out;
+  float* pq_w = nullptr;  // decoder: post_quant_conv [z, z] fp32, run on the caller's latent before conv_in
+  float* pq_b = nullptr;
+  LinW quant;             // encoder: quant_conv (1x1) after conv_out
+};
+
+// ---- CLIP text transformer (Hugging Face CLIPTextModel) ---------------------------------------------------------
 struct ClipLayerW {  // CLIPEncoderLayer: LN1 -> q|k|v -> causal attention -> out_proj (+x) -> LN2 -> fc1 -> act -> fc2 (+x)
   LinW qkv, out, fc1, fc2;   // layer_norm1 / layer_norm2 are folded into qkv / fc1
+};
+struct ClipW {
+  void* tok = nullptr;  // [vocab, C] 16-bit
+  void* pos = nullptr;  // [positions, C] 16-bit
+  std::vector<ClipLayerW> layers;
+  NormW final_norm;
 };
 
 struct Buf {
@@ -112,6 +165,7 @@ struct Act {  // NHWC 16-bit activation, row pitch == c
 };
 
 struct Plan;
+using KvKeys = std::vector<std::pair<std::string, int>>;  // (state-dict key, rows) of the batched cross-attention k|v
 
 }  // namespace
 
@@ -130,38 +184,10 @@ struct sdxe_engine {
   size_t cursor = 0;
   bool sizing = true;
 
-  // UNet
-  LinW te0, te2, le0, le2, emb_all;
-  int emb_total = 0;
-  // every transformer block's attn2.to_k / to_v stacked along N: the context is projected ONCE per UNet call
-  LinW kv_all;
-  int kv_total = 0;
-  std::vector<std::string> kv_keys;
-  std::vector<int> kv_rows;
-  std::vector<BlockW> in_blocks, out_blocks;
-  ResW mid_r1, mid_r2;
-  STW mid_st;
-  NormW out_norm;
-  LinW out_conv;
-  // VAE decoder
-  float* pq_w = nullptr;  // post_quant_conv [z, z] fp32
-  float* pq_b = nullptr;
-  LinW v_conv_in, v_conv_out, v_qkv, v_proj;
-  ResW v_mid1, v_mid2;
-  NormW v_attn_norm, v_norm_out;
-  std::vector<std::vector<ResW>> v_up_blocks;  // [level][block], level index as in the state dict
-  // VAE encoder (ldm Encoder: conv_in, down.{l}.block.{j} (+ downsample), mid, norm_out, conv_out; then quant_conv)
-  LinW e_conv_in, e_conv_out, e_qkv, e_proj, e_quant;
-  ResW e_mid1, e_mid2;
-  NormW e_attn_norm, e_norm_out;
-  std::vector<std::vector<ResW>> e_down_blocks;
-  std::vector<LinW> e_down_conv;
-  std::vector<LinW> v_up_conv;                    // per level (level 0 unused)
-  // CLIP text transformer
-  void* c_tok = nullptr;   // [vocab, C] 16-bit
-  void* c_pos = nullptr;   // [positions, C] 16-bit
-  std::vector<ClipLayerW> c_layers;
-  NormW c_final;
+  // the model's packed weights: exactly the one of cfg.kind is set (sdxe_create)
+  std::unique_ptr<UNetW> unet;
+  std::unique_ptr<VaeW> vae;  // decoder or encoder
+  std::unique_ptr<ClipW> clip;
 
   // activation pool
   std::multimap<size_t, void*> free_list;
@@ -171,13 +197,6 @@ struct sdxe_engine {
   // batches under s_min_uncond); every plan pins its own buffers (SDXL: > 100 MB of cross-attention k|v alone), so an
   // unbounded cache grows until cudaMalloc fails.
   std::map<std::string, std::unique_ptr<Plan>> plans;
-  // Cross-attention K / V cache: a non-zero key is the caller's promise that the context passed under that key always has
-  // the same contents (the conditioning of one job is step-invariant); a plan whose k|v buffer was last filled under the
-  // same key skips the context cast + projection GEMM (modules/sd_samplers_cfg_denoiser.py re-sends the same cond_in
-  // every sampler step).
-  int64_t ctx_key = 0;
-  // Hypertile rows (h', w', nh, nw, max_tiles) per attn1 layer for the next sdxe_unet_forward (sdxe_unet_set_hypertile)
-  std::vector<int32_t> ht_rows;
   // Circular padding in every 3x3 convolution with padding 1 (sdxe_set_circular): sticky, part of the plan key
   bool circular = false;
   int max_plans = 8;                    // sdxe_set_plan_cache
@@ -198,15 +217,18 @@ struct sdxe_engine {
   float* alloc32(size_t elems);
   int pack_linear(LinW& out, const std::vector<std::string>& wkeys, const std::vector<std::string>& bkeys, int n_each, int K,
                   int mode, int kpad = 0, int geglu_tile = 0);
+  int pack_dense(LinW& out, const std::string& prefix, int N, int K);     // <prefix>.weight [N, K] / .bias
+  int pack_conv3(LinW& out, const std::string& prefix, int N, int cin);  // <prefix>.weight [N, cin, 3, 3] / .bias
   int pack_norm(NormW& out, const std::string& prefix, int C);
   int fold_layer_norm(LinW& w, const NormW& ln);  // w consumes LayerNorm(ln) output: fold gamma / beta into w
   int pack_f32(float*& out, const std::string& key, int64_t n);
-  int build_unet();
-  int build_vae();
-  int build_vae_encoder();
-  int build_clip();
+  int build_unet(UNetW& u);
+  int build_vae_decoder(VaeW& v);
+  int build_vae_encoder(VaeW& v);
+  int build_clip(ClipW& c);
   int build_res(ResW& r, const std::string& p, int cin, int cout, const ResKeys& k);
-  int build_st(STW& s, const std::string& p, int C, int depth);
+  int build_st(UNetW& u, STW& s, const std::string& p, int C, int depth, KvKeys& kv);
+  int build_vae_mid(VaeMidW& m, const std::string& p, int C);
   // --- activations
   Buf alloc(size_t bytes);
   void release(Buf& b);
@@ -266,6 +288,9 @@ struct Builder {
   int ht_next = 0;
   // the plan's 3x3 convolutions with padding wrap around (torch padding_mode='circular') instead of reading zeros
   bool circular;
+  // UNet: the batched timestep-embedding rows every ResBlock adds after its first conv (null: none)
+  const float* emb = nullptr;
+  int ld_emb = 0;
 
   Builder(sdxe_engine* e_, Plan* p) : e(e_), plan(p), bf16(e_->bf16), ops(&p->body), circular(e_->circular) {}
 
@@ -459,8 +484,8 @@ struct Builder {
     Wk.K = kin;
     return gemm(col.p, kin, out.rows(), Wk, out.p, GemmOpt());
   }
-  // ldm Upsample: nearest 2x, then 3x3 conv; x is released
-  int upsample_conv(Act& x, const LinW& W, Act& out) {
+  // ldm Upsample: nearest 2x, then 3x3 conv; replaces x
+  int upsample_conv(Act& x, const LinW& W) {
     Act up = new_act(x.n, x.h * 2, x.w * 2, x.c);
     {
       const void* xp = x.p;
@@ -469,8 +494,8 @@ struct Builder {
       ops->push_back([=](cudaStream_t s) { return upsample2x_launch(xp, upp, n, h, w, c, s); });
     }
     free_act(x);
-    out = new_act(up.n, up.h, up.w, up.c);
-    ECHK(conv3(up, W, out.p, up.c, GemmOpt()));
+    x = new_act(up.n, up.h, up.w, up.c);
+    ECHK(conv3(up, W, x.p, up.c, GemmOpt()));
     free_act(up);
     return 0;
   }
@@ -493,13 +518,13 @@ struct Builder {
 
   // ---- UNet building blocks --------------------------------------------------------------------------------
   // ResBlock (ldm openaimodel.ResBlock, VAE ResnetBlock): GN32+SiLU -> conv3 (+emb) -> GN32+SiLU -> conv3 (+skip).
-  // emb_all: the UNet's batched timestep-embedding rows (null: none); skip_src: the UNet decoder's skip-concat input.
-  int res_block(const ResW& r, Act& x, Act* skip_src, const float* emb_all, int ld_emb, float eps, Act& out) {
+  // skip_src: the UNet decoder's skip-concat input.
+  int res_block(const ResW& r, const Act& x, Act* skip_src, float eps, Act& out) {
     Act g1;
     ECHK(group_norm(x, skip_src, r.n1, eps, true, g1));
     Act h = new_act(x.n, x.h, x.w, r.cout);
     GemmOpt o1;
-    if (emb_all) { o1.rowvec = emb_all + r.emb_off; o1.ldrv = ld_emb; o1.rows_per_sample = x.h * x.w; }
+    if (emb) { o1.rowvec = emb + r.emb_off; o1.ldrv = ld_emb; o1.rows_per_sample = x.h * x.w; }
     ECHK(conv3(g1, r.c1, h.p, r.cout, o1));
     free_act(g1);
     Act g2;
@@ -525,10 +550,18 @@ struct Builder {
     if (r.has_skip) free_act(sk);
     return 0;
   }
+  // a ResBlock whose input is not needed afterwards: replaces x
+  int res_replace(const ResW& r, Act& x, float eps, Act* skip_src = nullptr) {
+    Act out;
+    ECHK(res_block(r, x, skip_src, eps, out));
+    free_act(x);
+    x = out;
+    return 0;
+  }
 
-  // SpatialTransformer (modules/sd_hijack_unet.py:83-102) with BasicTransformerBlocks
+  // SpatialTransformer (modules/sd_hijack_unet.py:83-102) with BasicTransformerBlocks; replaces x
   // kv_all: [B * ctx_len, ld_kv] = every block's cross-attention k | v projection of the context (one GEMM per call)
-  int spatial_transformer(const STW& st, Act& x, const void* kv_all, int ld_kv, int ctx_len, Act& out) {
+  int spatial_transformer(const STW& st, Act& x, const void* kv_all, int ld_kv, int ctx_len) {
     const int C = st.C, H = st.heads, dh = st.dh;
     const int64_t M = x.rows();
     const int tokens = x.h * x.w, B = x.n;
@@ -618,12 +651,40 @@ struct Builder {
       free_act(h);
       h = h4;
     }
-    out = new_act(x.n, x.h, x.w, C);
+    Act out = new_act(x.n, x.h, x.w, C);
     GemmOpt op;
     op.residual = x.p; op.ldr = C;
     ECHK(gemm(h.p, C, M, st.proj_out, out.p, op));
     free_act(h);
+    free_act(x);
+    x = out;
     return 0;
+  }
+
+  // ---- VAE building blocks ---------------------------------------------------------------------------------
+  // mid block: ResBlock -> AttnBlock (sd_hijack_optimizations.py:637-655) -> ResBlock; replaces cur
+  int vae_mid(const VaeMidW& m, Act& cur) {
+    ECHK(res_replace(m.r1, cur, 1e-6f));
+    const int C = cur.c, tokens = cur.h * cur.w, n = cur.n;
+    const int64_t M = cur.rows();
+    Act xn;
+    ECHK(group_norm(cur, nullptr, m.attn_norm, 1e-6f, false, xn));
+    Buf qkv = e->alloc((size_t)M * 3 * C * 2);
+    ECHK(gemm(xn.p, C, M, m.qkv, qkv.p, GemmOpt()));
+    free_act(xn);
+    if (C % 64 != 0 || C > 512) EFAIL("vae attention: channel count must be a multiple of 64 and <= 512");
+    Act att = new_act(n, cur.h, cur.w, C);
+    const uint16_t* qp = (const uint16_t*)qkv.p;
+    ECHK(attention(qp, qp + C, qp + 2 * C, n, 1, tokens, tokens, C, 3 * C, 3 * C, 1.0f / sqrtf((float)C), att.p, C, C));
+    e->release(qkv);
+    Act o = new_act(n, cur.h, cur.w, C);
+    GemmOpt op;
+    op.residual = cur.p; op.ldr = C;
+    ECHK(gemm(att.p, C, M, m.proj, o.p, op));
+    free_act(att);
+    free_act(cur);
+    cur = o;
+    return res_replace(m.r2, cur, 1e-6f);
   }
 };
 
@@ -650,7 +711,6 @@ const RawWeight* sdxe_engine::find(const std::string& key, int64_t numel) {
     if (missing.size() < 600) missing += (missing.empty() ? "" : ", ") + key + "(shape)";
     return nullptr;
   }
-  it->second.used = true;
   return &it->second;
 }
 void* sdxe_engine::alloc16(size_t elems) {
@@ -728,29 +788,38 @@ static int conv_kpad(int cin) {
   const int k = 9 * cin;
   return (cin % 64 == 0) ? k : (int)align_up(k, 64);
 }
+int sdxe_engine::pack_dense(LinW& out, const std::string& prefix, int N, int K) {
+  return pack_linear(out, {prefix + ".weight"}, {prefix + ".bias"}, N, K, PACK_PLAIN);
+}
+int sdxe_engine::pack_conv3(LinW& out, const std::string& prefix, int N, int cin) {
+  return pack_linear(out, {prefix + ".weight"}, {prefix + ".bias"}, N, 9 * cin, PACK_CONV3, conv_kpad(cin));
+}
 
 int sdxe_engine::build_res(ResW& r, const std::string& p, int cin, int cout, const ResKeys& k) {
   r.cin = cin; r.cout = cout;
-  const std::string c1 = p + k.c1, c2 = p + k.c2, sk = p + k.skip;
   ECHK(pack_norm(r.n1, p + k.n1, cin));
-  ECHK(pack_linear(r.c1, {c1 + ".weight"}, {c1 + ".bias"}, cout, 9 * cin, PACK_CONV3, conv_kpad(cin)));
+  ECHK(pack_conv3(r.c1, p + k.c1, cout, cin));
   ECHK(pack_norm(r.n2, p + k.n2, cout));
-  ECHK(pack_linear(r.c2, {c2 + ".weight"}, {c2 + ".bias"}, cout, 9 * cout, PACK_CONV3, conv_kpad(cout)));
+  ECHK(pack_conv3(r.c2, p + k.c2, cout, cout));
   r.has_skip = cin != cout;
-  if (r.has_skip) ECHK(pack_linear(r.skip, {sk + ".weight"}, {sk + ".bias"}, cout, cin, PACK_PLAIN));
+  if (r.has_skip) ECHK(pack_dense(r.skip, p + k.skip, cout, cin));
   return 0;
 }
 
-int sdxe_engine::build_st(STW& s, const std::string& p, int C, int depth) {
+// =================================================================================================================
+// UNet weights
+// =================================================================================================================
+// kv: the blocks' cross-attention k / v keys, packed as one matrix after every block is known (build_unet)
+int sdxe_engine::build_st(UNetW& u, STW& s, const std::string& p, int C, int depth, KvKeys& kv) {
   s.C = C;
   if (cfg.num_head_channels > 0) { s.dh = cfg.num_head_channels; s.heads = C / s.dh; }
   else { s.heads = cfg.num_heads; s.dh = C / s.heads; }
   if (s.dh % 8) EFAIL("head dim must be a multiple of 8");
-  const int ctx = cfg.context_dim;
   ECHK(pack_norm(s.gn, p + ".norm", C));
-  ECHK(pack_linear(s.proj_in, {p + ".proj_in.weight"}, {p + ".proj_in.bias"}, C, C, PACK_PLAIN));
-  ECHK(pack_linear(s.proj_out, {p + ".proj_out.weight"}, {p + ".proj_out.bias"}, C, C, PACK_PLAIN));
+  ECHK(pack_dense(s.proj_in, p + ".proj_in", C, C));
+  ECHK(pack_dense(s.proj_out, p + ".proj_out", C, C));
   s.blocks.resize(depth);
+  u.n_attn1 += depth;
   for (int j = 0; j < depth; ++j) {
     TBlockW& t = s.blocks[j];
     const std::string b = p + ".transformer_blocks." + std::to_string(j);
@@ -758,17 +827,17 @@ int sdxe_engine::build_st(STW& s, const std::string& p, int C, int depth) {
     ECHK(pack_norm(t.ln2, b + ".norm2", C));
     ECHK(pack_norm(t.ln3, b + ".norm3", C));
     ECHK(pack_linear(t.qkv1, {b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"}, {}, C, C, PACK_PLAIN));
-    ECHK(pack_linear(t.out1, {b + ".attn1.to_out.0.weight"}, {b + ".attn1.to_out.0.bias"}, C, C, PACK_PLAIN));
+    ECHK(pack_dense(t.out1, b + ".attn1.to_out.0", C, C));
     ECHK(pack_linear(t.q2, {b + ".attn2.to_q.weight"}, {}, C, C, PACK_PLAIN));
-    t.kv_off = kv_total;  // packed after all blocks are known (build_unet)
-    kv_keys.push_back(b + ".attn2.to_k.weight"); kv_rows.push_back(C);
-    kv_keys.push_back(b + ".attn2.to_v.weight"); kv_rows.push_back(C);
-    kv_total += 2 * C;
-    ECHK(pack_linear(t.out2, {b + ".attn2.to_out.0.weight"}, {b + ".attn2.to_out.0.bias"}, C, C, PACK_PLAIN));
+    t.kv_off = u.kv_total;
+    kv.push_back({b + ".attn2.to_k.weight", C});
+    kv.push_back({b + ".attn2.to_v.weight", C});
+    u.kv_total += 2 * C;
+    ECHK(pack_dense(t.out2, b + ".attn2.to_out.0", C, C));
     const int n1 = 8 * C;
     const int tile = n1 % 256 == 0 ? 256 : (n1 % 128 == 0 ? 128 : 64);
     ECHK(pack_linear(t.ff1, {b + ".ff.net.0.proj.weight"}, {b + ".ff.net.0.proj.bias"}, n1, C, PACK_GEGLU, 0, tile));
-    ECHK(pack_linear(t.ff2, {b + ".ff.net.2.weight"}, {b + ".ff.net.2.bias"}, C, 4 * C, PACK_PLAIN));
+    ECHK(pack_dense(t.ff2, b + ".ff.net.2", C, 4 * C));
     // norm1 / norm2 / norm3 are folded into the GEMMs that consume them (no LayerNorm kernel runs)
     ECHK(fold_layer_norm(t.qkv1, t.ln1));
     ECHK(fold_layer_norm(t.q2, t.ln2));
@@ -777,224 +846,186 @@ int sdxe_engine::build_st(STW& s, const std::string& p, int C, int depth) {
   return 0;
 }
 
-int sdxe_engine::build_unet() {
+int sdxe_engine::build_unet(UNetW& u) {
   const int mc = cfg.model_channels, ted = 4 * mc, nl = cfg.num_levels, nrb = cfg.num_res_blocks;
-  ECHK(pack_linear(te0, {"time_embed.0.weight"}, {"time_embed.0.bias"}, ted, mc, PACK_PLAIN));
-  ECHK(pack_linear(te2, {"time_embed.2.weight"}, {"time_embed.2.bias"}, ted, ted, PACK_PLAIN));
+  ECHK(pack_dense(u.te0, "time_embed.0", ted, mc));
+  ECHK(pack_dense(u.te2, "time_embed.2", ted, ted));
   if (cfg.adm_in_channels > 0) {
-    ECHK(pack_linear(le0, {"label_emb.0.0.weight"}, {"label_emb.0.0.bias"}, ted, cfg.adm_in_channels, PACK_PLAIN));
-    ECHK(pack_linear(le2, {"label_emb.0.2.weight"}, {"label_emb.0.2.bias"}, ted, ted, PACK_PLAIN));
+    ECHK(pack_dense(u.le0, "label_emb.0.0", ted, cfg.adm_in_channels));
+    ECHK(pack_dense(u.le2, "label_emb.0.2", ted, ted));
   }
-  in_blocks.clear(); out_blocks.clear();
-  kv_keys.clear(); kv_rows.clear(); kv_total = 0;
+  u.in_levels.assign(nl, {});
+  u.out_blocks.clear();
+  u.kv_total = u.n_attn1 = 0;
+  KvKeys kv;
   std::vector<std::string> emb_w, emb_b;  // batched emb_layers (every ResBlock's Linear(SiLU(emb)) in one skinny GEMM)
   std::vector<int> emb_n;
   int emb_cursor = 0;
-  auto add_emb = [&](ResW& r, const std::string& p) {
+  auto add_res = [&](ResW& r, const std::string& p, int cin, int cout) {
+    ECHK(build_res(r, p, cin, cout, UNET_RES));
     r.emb_off = emb_cursor;
     emb_cursor += r.cout;
     emb_w.push_back(p + ".emb_layers.1.weight");
     emb_b.push_back(p + ".emb_layers.1.bias");
     emb_n.push_back(r.cout);
+    return 0;
   };
-  {
-    BlockW b0;
-    b0.kind = 0;
-    ECHK(pack_linear(b0.conv_in, {"input_blocks.0.0.weight"}, {"input_blocks.0.0.bias"}, mc, 9 * cfg.in_channels, PACK_CONV3,
-                     conv_kpad(cfg.in_channels)));
-    b0.ch_out = mc;
-    in_blocks.push_back(b0);
-  }
+  ECHK(pack_conv3(u.conv_in, "input_blocks.0.0", mc, cfg.in_channels));
   std::vector<int> chans = {mc};
   int ch = mc, idx = 1;
   for (int level = 0; level < nl; ++level) {
     const int mult = cfg.channel_mult[level];
-    for (int r = 0; r < nrb; ++r) {
-      BlockW b;
-      b.kind = 1;
-      const std::string p = "input_blocks." + std::to_string(idx);
-      ECHK(build_res(b.res, p + ".0", ch, mult * mc, UNET_RES));
-      add_emb(b.res, p + ".0");
+    UNetLevelW& lv = u.in_levels[level];
+    lv.blocks.resize(nrb);
+    for (UNetBlockW& b : lv.blocks) {
+      const std::string p = "input_blocks." + std::to_string(idx++);
+      ECHK(add_res(b.res, p + ".0", ch, mult * mc));
       ch = mult * mc;
-      if (cfg.transformer_depth[level] > 0) {
-        b.has_st = true;
-        ECHK(build_st(b.st, p + ".1", ch, cfg.transformer_depth[level]));
-      }
-      b.ch_out = ch;
-      in_blocks.push_back(b);
+      b.has_st = cfg.transformer_depth[level] > 0;
+      if (b.has_st) ECHK(build_st(u, b.st, p + ".1", ch, cfg.transformer_depth[level], kv));
       chans.push_back(ch);
-      ++idx;
     }
-    if (level != nl - 1) {
-      BlockW b;
-      b.kind = 2;
-      const std::string p = "input_blocks." + std::to_string(idx) + ".0.op";
-      ECHK(pack_linear(b.down, {p + ".weight"}, {p + ".bias"}, ch, 9 * ch, PACK_CONV3, conv_kpad(ch)));
-      b.ch_out = ch;
-      in_blocks.push_back(b);
+    lv.has_down = level != nl - 1;
+    if (lv.has_down) {
+      ECHK(pack_conv3(lv.down, "input_blocks." + std::to_string(idx++) + ".0.op", ch, ch));
       chans.push_back(ch);
-      ++idx;
     }
   }
-  ECHK(build_res(mid_r1, "middle_block.0", ch, ch, UNET_RES));
-  add_emb(mid_r1, "middle_block.0");
-  ECHK(build_st(mid_st, "middle_block.1", ch, std::max(1, cfg.transformer_depth_middle)));
-  ECHK(build_res(mid_r2, "middle_block.2", ch, ch, UNET_RES));
-  add_emb(mid_r2, "middle_block.2");
+  ECHK(add_res(u.mid_r1, "middle_block.0", ch, ch));
+  ECHK(build_st(u, u.mid_st, "middle_block.1", ch, std::max(1, cfg.transformer_depth_middle), kv));
+  ECHK(add_res(u.mid_r2, "middle_block.2", ch, ch));
   idx = 0;
   for (int level = nl - 1; level >= 0; --level) {
     const int mult = cfg.channel_mult[level];
     for (int i = 0; i <= nrb; ++i) {
       const int ich = chans.back();
       chans.pop_back();
-      BlockW b;
-      b.kind = 1;
-      const std::string p = "output_blocks." + std::to_string(idx);
-      ECHK(build_res(b.res, p + ".0", ch + ich, mc * mult, UNET_RES));
-      add_emb(b.res, p + ".0");
+      UNetBlockW b;
+      const std::string p = "output_blocks." + std::to_string(idx++);
+      ECHK(add_res(b.res, p + ".0", ch + ich, mc * mult));
       ch = mc * mult;
-      int sub = 1;
-      if (cfg.transformer_depth[level] > 0) {
-        b.has_st = true;
-        ECHK(build_st(b.st, p + ".1", ch, cfg.transformer_depth[level]));
-        sub = 2;
-      }
-      if (level && i == nrb) {
-        b.has_up = true;
-        const std::string u = p + "." + std::to_string(sub) + ".conv";
-        ECHK(pack_linear(b.up, {u + ".weight"}, {u + ".bias"}, ch, 9 * ch, PACK_CONV3, conv_kpad(ch)));
-      }
-      b.ch_out = ch;
-      out_blocks.push_back(b);
-      ++idx;
+      b.has_st = cfg.transformer_depth[level] > 0;
+      if (b.has_st) ECHK(build_st(u, b.st, p + ".1", ch, cfg.transformer_depth[level], kv));
+      b.has_up = level && i == nrb;
+      if (b.has_up) ECHK(pack_conv3(b.up, p + "." + std::to_string(b.has_st ? 2 : 1) + ".conv", ch, ch));
+      u.out_blocks.push_back(b);
     }
   }
-  ECHK(pack_norm(out_norm, "out.0", ch));
-  ECHK(pack_linear(out_conv, {"out.2.weight"}, {"out.2.bias"}, cfg.out_channels, 9 * ch, PACK_CONV3, conv_kpad(ch)));
+  ECHK(pack_norm(u.out_norm, "out.0", ch));
+  ECHK(pack_conv3(u.out_conv, "out.2", cfg.out_channels, ch));
   // batched emb_layers: rows of different widths -> pack key by key
-  emb_total = emb_cursor;
-  emb_all.N = emb_total; emb_all.K = ted; emb_all.ld = ted;
-  emb_all.w = alloc16((size_t)emb_total * ted);
-  emb_all.b = alloc32(align_up((size_t)emb_total, 8));
+  u.emb_total = emb_cursor;
+  LinW& ea = u.emb_all;
+  ea.N = u.emb_total; ea.K = ted; ea.ld = ted;
+  ea.w = alloc16((size_t)u.emb_total * ted);
+  ea.b = alloc32(align_up((size_t)u.emb_total, 8));
   int off = 0;
   for (size_t i = 0; i < emb_w.size(); ++i) {
     const RawWeight* w = find(emb_w[i], (int64_t)emb_n[i] * ted);
     const RawWeight* b = find(emb_b[i], emb_n[i]);
     if (!sizing && w && b) {
-      ECHK(pack_weight_launch(w->dev, w->dtype, (char*)emb_all.w + (size_t)off * ted * 2, PACK_PLAIN, emb_n[i], ted, ted, 0, bf16, 0));
-      ECHK(pack_vector_launch(b->dev, b->dtype, emb_all.b + off, emb_n[i], 0, true, bf16, 0));
+      ECHK(pack_weight_launch(w->dev, w->dtype, (char*)ea.w + (size_t)off * ted * 2, PACK_PLAIN, emb_n[i], ted, ted, 0, bf16, 0));
+      ECHK(pack_vector_launch(b->dev, b->dtype, ea.b + off, emb_n[i], 0, true, bf16, 0));
     }
     off += emb_n[i];
   }
   // batched cross-attention K/V projection weights [kv_total, context_dim]
-  {
-    const int ctx = cfg.context_dim;
-    kv_all.N = kv_total; kv_all.K = ctx; kv_all.ld = ctx; kv_all.b = nullptr;
-    kv_all.Nrows = (int)align_up((size_t)kv_total, 16);
-    kv_all.w = alloc16((size_t)kv_all.Nrows * ctx);
-    int row = 0;
-    for (size_t i = 0; i < kv_keys.size(); ++i) {
-      const RawWeight* w = find(kv_keys[i], (int64_t)kv_rows[i] * ctx);
-      if (!sizing && w)
-        ECHK(pack_weight_launch(w->dev, w->dtype, (char*)kv_all.w + (size_t)row * ctx * 2, PACK_PLAIN, kv_rows[i], ctx, ctx, 0, bf16, 0));
-      row += kv_rows[i];
-    }
+  const int ctx = cfg.context_dim;
+  LinW& kva = u.kv_all;
+  kva.N = u.kv_total; kva.K = ctx; kva.ld = ctx; kva.b = nullptr;
+  kva.Nrows = (int)align_up((size_t)u.kv_total, 16);
+  kva.w = alloc16((size_t)kva.Nrows * ctx);
+  int row = 0;
+  for (const auto& k : kv) {
+    const RawWeight* w = find(k.first, (int64_t)k.second * ctx);
+    if (!sizing && w)
+      ECHK(pack_weight_launch(w->dev, w->dtype, (char*)kva.w + (size_t)row * ctx * 2, PACK_PLAIN, k.second, ctx, ctx, 0, bf16, 0));
+    row += k.second;
   }
   return 0;
 }
 
-int sdxe_engine::build_vae() {
+// =================================================================================================================
+// VAE weights
+// =================================================================================================================
+int sdxe_engine::build_vae_mid(VaeMidW& m, const std::string& p, int C) {
+  const std::string a = p + ".attn_1.";
+  ECHK(build_res(m.r1, p + ".block_1", C, C, VAE_RES));
+  ECHK(pack_norm(m.attn_norm, a + "norm", C));
+  ECHK(pack_linear(m.qkv, {a + "q.weight", a + "k.weight", a + "v.weight"}, {a + "q.bias", a + "k.bias", a + "v.bias"}, C, C, PACK_PLAIN));
+  ECHK(pack_dense(m.proj, a + "proj_out", C, C));
+  return build_res(m.r2, p + ".block_2", C, C, VAE_RES);
+}
+
+int sdxe_engine::build_vae_decoder(VaeW& v) {
   const int z = cfg.vae_z_channels, nl = cfg.num_levels, nrb = cfg.num_res_blocks;
-  ECHK(pack_f32(pq_w, "post_quant_conv.weight", (int64_t)z * z));
-  ECHK(pack_f32(pq_b, "post_quant_conv.bias", z));
+  ECHK(pack_f32(v.pq_w, "post_quant_conv.weight", (int64_t)z * z));
+  ECHK(pack_f32(v.pq_b, "post_quant_conv.bias", z));
   int bi = cfg.vae_ch * cfg.channel_mult[nl - 1];
-  ECHK(pack_linear(v_conv_in, {"decoder.conv_in.weight"}, {"decoder.conv_in.bias"}, bi, 9 * z, PACK_CONV3, conv_kpad(z)));
-  ECHK(build_res(v_mid1, "decoder.mid.block_1", bi, bi, VAE_RES));
-  ECHK(pack_norm(v_attn_norm, "decoder.mid.attn_1.norm", bi));
-  ECHK(pack_linear(v_qkv, {"decoder.mid.attn_1.q.weight", "decoder.mid.attn_1.k.weight", "decoder.mid.attn_1.v.weight"},
-                   {"decoder.mid.attn_1.q.bias", "decoder.mid.attn_1.k.bias", "decoder.mid.attn_1.v.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(pack_linear(v_proj, {"decoder.mid.attn_1.proj_out.weight"}, {"decoder.mid.attn_1.proj_out.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(build_res(v_mid2, "decoder.mid.block_2", bi, bi, VAE_RES));
-  v_up_blocks.assign(nl, {});
-  v_up_conv.assign(nl, LinW());
+  ECHK(pack_conv3(v.conv_in, "decoder.conv_in", bi, z));
+  ECHK(build_vae_mid(v.mid, "decoder.mid", bi));
+  v.levels.assign(nl, {});
   for (int level = nl - 1; level >= 0; --level) {
+    VaeLevelW& lv = v.levels[level];
+    const std::string p = "decoder.up." + std::to_string(level);
     const int bo = cfg.vae_ch * cfg.channel_mult[level];
-    for (int j = 0; j <= nrb; ++j) {
-      ResW r;
-      ECHK(build_res(r, "decoder.up." + std::to_string(level) + ".block." + std::to_string(j), bi, bo, VAE_RES));
-      v_up_blocks[level].push_back(r);
-      bi = bo;
-    }
-    if (level != 0) {
-      const std::string u = "decoder.up." + std::to_string(level) + ".upsample.conv";
-      ECHK(pack_linear(v_up_conv[level], {u + ".weight"}, {u + ".bias"}, bi, 9 * bi, PACK_CONV3, conv_kpad(bi)));
-    }
+    lv.blocks.resize(nrb + 1);
+    for (int j = 0; j <= nrb; ++j, bi = bo) ECHK(build_res(lv.blocks[j], p + ".block." + std::to_string(j), bi, bo, VAE_RES));
+    lv.has_resample = level != 0;
+    if (lv.has_resample) ECHK(pack_conv3(lv.resample, p + ".upsample.conv", bi, bi));
   }
-  ECHK(pack_norm(v_norm_out, "decoder.norm_out", bi));
-  ECHK(pack_linear(v_conv_out, {"decoder.conv_out.weight"}, {"decoder.conv_out.bias"}, cfg.vae_out_ch, 9 * bi, PACK_CONV3, conv_kpad(bi)));
-  return 0;
+  ECHK(pack_norm(v.norm_out, "decoder.norm_out", bi));
+  return pack_conv3(v.conv_out, "decoder.conv_out", cfg.vae_out_ch, bi);
 }
 
-int sdxe_engine::build_vae_encoder() {
-  const int z = cfg.vae_z_channels, nl = cfg.num_levels, nrb = cfg.num_res_blocks, ch = cfg.vae_ch, cin = cfg.vae_out_ch;
-  ECHK(pack_linear(e_conv_in, {"encoder.conv_in.weight"}, {"encoder.conv_in.bias"}, ch, 9 * cin, PACK_CONV3, conv_kpad(cin)));
-  e_down_blocks.assign(nl, {});
-  e_down_conv.assign(nl, LinW());
+int sdxe_engine::build_vae_encoder(VaeW& v) {
+  const int z = cfg.vae_z_channels, nl = cfg.num_levels, nrb = cfg.num_res_blocks, ch = cfg.vae_ch;
+  ECHK(pack_conv3(v.conv_in, "encoder.conv_in", ch, cfg.vae_out_ch));
+  v.levels.assign(nl, {});
   int bi = ch;
   for (int level = 0; level < nl; ++level) {
+    VaeLevelW& lv = v.levels[level];
+    const std::string p = "encoder.down." + std::to_string(level);
     const int bo = ch * cfg.channel_mult[level];
-    for (int j = 0; j < nrb; ++j) {
-      ResW r;
-      ECHK(build_res(r, "encoder.down." + std::to_string(level) + ".block." + std::to_string(j), bi, bo, VAE_RES));
-      e_down_blocks[level].push_back(r);
-      bi = bo;
-    }
-    if (level != nl - 1) {
-      const std::string d = "encoder.down." + std::to_string(level) + ".downsample.conv";
-      ECHK(pack_linear(e_down_conv[level], {d + ".weight"}, {d + ".bias"}, bi, 9 * bi, PACK_CONV3, conv_kpad(bi)));
-    }
+    lv.blocks.resize(nrb);
+    for (int j = 0; j < nrb; ++j, bi = bo) ECHK(build_res(lv.blocks[j], p + ".block." + std::to_string(j), bi, bo, VAE_RES));
+    lv.has_resample = level != nl - 1;
+    if (lv.has_resample) ECHK(pack_conv3(lv.resample, p + ".downsample.conv", bi, bi));
   }
-  ECHK(build_res(e_mid1, "encoder.mid.block_1", bi, bi, VAE_RES));
-  ECHK(pack_norm(e_attn_norm, "encoder.mid.attn_1.norm", bi));
-  ECHK(pack_linear(e_qkv, {"encoder.mid.attn_1.q.weight", "encoder.mid.attn_1.k.weight", "encoder.mid.attn_1.v.weight"},
-                   {"encoder.mid.attn_1.q.bias", "encoder.mid.attn_1.k.bias", "encoder.mid.attn_1.v.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(pack_linear(e_proj, {"encoder.mid.attn_1.proj_out.weight"}, {"encoder.mid.attn_1.proj_out.bias"}, bi, bi, PACK_PLAIN));
-  ECHK(build_res(e_mid2, "encoder.mid.block_2", bi, bi, VAE_RES));
-  ECHK(pack_norm(e_norm_out, "encoder.norm_out", bi));
-  ECHK(pack_linear(e_conv_out, {"encoder.conv_out.weight"}, {"encoder.conv_out.bias"}, 2 * z, 9 * bi, PACK_CONV3, conv_kpad(bi)));
-  ECHK(pack_linear(e_quant, {"quant_conv.weight"}, {"quant_conv.bias"}, 2 * z, 2 * z, PACK_PLAIN));
-  return 0;
+  ECHK(build_vae_mid(v.mid, "encoder.mid", bi));
+  ECHK(pack_norm(v.norm_out, "encoder.norm_out", bi));
+  ECHK(pack_conv3(v.conv_out, "encoder.conv_out", 2 * z, bi));
+  return pack_dense(v.quant, "quant_conv", 2 * z, 2 * z);
 }
 
 // =================================================================================================================
 // CLIP text transformer weights (Hugging Face CLIPTextModel names; open_clip towers are renamed on the host)
 // =================================================================================================================
-int sdxe_engine::build_clip() {
+int sdxe_engine::build_clip(ClipW& c) {
   const int C = cfg.clip_hidden, I = cfg.clip_intermediate, L = cfg.clip_layers;
   const std::string tm = "text_model.";
-  c_tok = alloc16((size_t)cfg.clip_vocab * C);
-  c_pos = alloc16((size_t)cfg.clip_positions * C);
+  c.tok = alloc16((size_t)cfg.clip_vocab * C);
+  c.pos = alloc16((size_t)cfg.clip_positions * C);
   const RawWeight* wt = find(tm + "embeddings.token_embedding.weight", (int64_t)cfg.clip_vocab * C);
   const RawWeight* wp = find(tm + "embeddings.position_embedding.weight", (int64_t)cfg.clip_positions * C);
-  if (!sizing && wt) ECHK(pack_weight_launch(wt->dev, wt->dtype, c_tok, PACK_PLAIN, cfg.clip_vocab, C, C, 0, bf16, 0));
-  if (!sizing && wp) ECHK(pack_weight_launch(wp->dev, wp->dtype, c_pos, PACK_PLAIN, cfg.clip_positions, C, C, 0, bf16, 0));
-  c_layers.resize(L);
+  if (!sizing && wt) ECHK(pack_weight_launch(wt->dev, wt->dtype, c.tok, PACK_PLAIN, cfg.clip_vocab, C, C, 0, bf16, 0));
+  if (!sizing && wp) ECHK(pack_weight_launch(wp->dev, wp->dtype, c.pos, PACK_PLAIN, cfg.clip_positions, C, C, 0, bf16, 0));
+  c.layers.resize(L);
   for (int l = 0; l < L; ++l) {
-    ClipLayerW& w = c_layers[l];
+    ClipLayerW& w = c.layers[l];
     const std::string p = tm + "encoder.layers." + std::to_string(l) + ".";
     NormW ln1, ln2;
     ECHK(pack_norm(ln1, p + "layer_norm1", C));
     ECHK(pack_norm(ln2, p + "layer_norm2", C));
     ECHK(pack_linear(w.qkv, {p + "self_attn.q_proj.weight", p + "self_attn.k_proj.weight", p + "self_attn.v_proj.weight"},
                      {p + "self_attn.q_proj.bias", p + "self_attn.k_proj.bias", p + "self_attn.v_proj.bias"}, C, C, PACK_PLAIN));
-    ECHK(pack_linear(w.out, {p + "self_attn.out_proj.weight"}, {p + "self_attn.out_proj.bias"}, C, C, PACK_PLAIN));
-    ECHK(pack_linear(w.fc1, {p + "mlp.fc1.weight"}, {p + "mlp.fc1.bias"}, I, C, PACK_PLAIN));
-    ECHK(pack_linear(w.fc2, {p + "mlp.fc2.weight"}, {p + "mlp.fc2.bias"}, C, I, PACK_PLAIN));
+    ECHK(pack_dense(w.out, p + "self_attn.out_proj", C, C));
+    ECHK(pack_dense(w.fc1, p + "mlp.fc1", I, C));
+    ECHK(pack_dense(w.fc2, p + "mlp.fc2", C, I));
     ECHK(fold_layer_norm(w.qkv, ln1));
     ECHK(fold_layer_norm(w.fc1, ln2));
   }
-  ECHK(pack_norm(c_final, tm + "final_layer_norm", C));
-  return 0;
+  return pack_norm(c.final_norm, tm + "final_layer_norm", C);
 }
 
 // =================================================================================================================
@@ -1105,6 +1136,7 @@ int run_ops_profiled(sdxe_engine* e, std::vector<OpRec>& ops, cudaStream_t s) {
 // ---- UNet plan -----------------------------------------------------------------------------------------------
 int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len, const std::vector<int32_t>* ht) {
   const sdxe_config& cfg = e->cfg;
+  const UNetW& u = *e->unet;
   Builder B(e, p);
   const bool bf16 = e->bf16;
   const int mc = cfg.model_channels, ted = 4 * mc;
@@ -1132,11 +1164,11 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len, c
   }
   // ---- embeddings (fp32 vectors rounded through the 16-bit type where the reference's autocast rounds)
   Buf e1 = e->alloc(sizeof(float) * n * ted), emb = e->alloc(sizeof(float) * n * ted), l1 = e->alloc(sizeof(float) * n * ted);
-  Buf emb_all = e->alloc(sizeof(float) * n * e->emb_total);
+  Buf emb_all = e->alloc(sizeof(float) * n * u.emb_total);
   {
-    const LinW te0 = e->te0, te2 = e->te2, le0 = e->le0, le2 = e->le2, ea = e->emb_all;
+    const LinW te0 = u.te0, te2 = u.te2, le0 = u.le0, le2 = u.le2, ea = u.emb_all;
     float *pt = (float*)temb.p, *p1 = (float*)e1.p, *pe = (float*)emb.p, *pl = (float*)l1.p, *pa = (float*)emb_all.p, *py = (float*)y32.p;
-    const int adm = cfg.adm_in_channels, etot = e->emb_total;
+    const int adm = cfg.adm_in_channels, etot = u.emb_total;
     // time_embed = Linear -> SiLU -> Linear; every consumer of `emb` (the ResBlocks' emb_layers) applies SiLU first,
     // so the SiLU'd vector is what gets stored (rounded through the 16-bit type at each step like the reference).
     B.ops->push_back([=](cudaStream_t s) { return skinny_linear_launch(pt, mc, te0.w, te0.b, nullptr, p1, ted, n, ted, mc, true, bf16, s); });
@@ -1150,94 +1182,72 @@ int build_unet_plan(sdxe_engine* e, Plan* p, int n, int h, int w, int ctx_len, c
     }
     B.ops->push_back([=](cudaStream_t s) { return skinny_linear_launch(pe, ted, ea.w, ea.b, nullptr, pa, etot, n, etot, ted, false, bf16, s); });
   }
-  const float* emb_ptr = (const float*)emb_all.p;
-  const int ld_emb = e->emb_total;
+  B.emb = (const float*)emb_all.p;
+  B.ld_emb = u.emb_total;
   // ---- cross-attention keys / values of ALL transformer blocks: one GEMM over the context (plan-owned buffer)
-  Buf kvbuf = e->alloc((size_t)n * ctx_len * std::max(8, e->kv_total) * 2);
+  Buf kvbuf = e->alloc((size_t)n * ctx_len * std::max(8, u.kv_total) * 2);
   {
     // runs before the graph, and only when the context changed (ctx_key): cast the caller's context, project it once
     auto kv_ops = std::make_shared<std::vector<OpRec>>();
-    if (e->kv_total > 0) {
+    if (u.kv_total > 0) {
       B.ops = kv_ops.get();
-      const int rc = B.gemm(ctx16.p, cfg.context_dim, (int64_t)n * ctx_len, e->kv_all, kvbuf.p, Builder::GemmOpt());
+      const int rc = B.gemm(ctx16.p, cfg.context_dim, (int64_t)n * ctx_len, u.kv_all, kvbuf.p, Builder::GemmOpt());
       B.ops = &p->body;
       ECHK(rc);
     }
     void* cx = ctx16.p;
     const int cdim = cfg.context_dim;
+    const UNetW* up = &u;
     p->pre.push_back([=](cudaStream_t s) {
-      if (e->ctx_key != 0 && p->kv_key == e->ctx_key && !e->profiling) return 0;
+      if (up->ctx_key != 0 && p->kv_key == up->ctx_key && !e->profiling) return 0;
       ECHK(cast_rows_launch(p->ctx, p->io_dtype, cx, (int64_t)n * ctx_len, cdim, cdim, bf16, s));
       if (e->profiling) ECHK(run_ops_profiled(e, *kv_ops, s));
       else ECHK(run_ops(*kv_ops, s));
-      p->kv_key = e->ctx_key;
+      p->kv_key = up->ctx_key;
       return 0;
     });
   }
+  auto transformer = [&](const UNetBlockW& b, Act& x) { return b.has_st ? B.spatial_transformer(b.st, x, kvbuf.p, u.kv_total, ctx_len) : 0; };
 
-  // ---- input blocks
+  // ---- input blocks; every output stays alive on the skip stack
   std::vector<Act> hs;
   Act cur;
-  for (size_t bi = 0; bi < e->in_blocks.size(); ++bi) {
-    const BlockW& b = e->in_blocks[bi];
-    if (b.kind == 0) {
-      ECHK(B.conv_in_nchw(nullptr, n, cfg.in_channels, h, w, b.conv_in, cur));
-    } else if (b.kind == 1) {
+  ECHK(B.conv_in_nchw(nullptr, n, cfg.in_channels, h, w, u.conv_in, cur));
+  hs.push_back(cur);
+  for (const UNetLevelW& lv : u.in_levels) {
+    for (const UNetBlockW& b : lv.blocks) {
       Act r;
-      ECHK(B.res_block(b.res, cur, nullptr, emb_ptr, ld_emb, 1e-5f, r));
-      // `cur` stays alive: it is on the skip stack
-      if (b.has_st) {
-        Act t;
-        ECHK(B.spatial_transformer(b.st, r, kvbuf.p, e->kv_total, ctx_len, t));
-        B.free_act(r);
-        r = t;
-      }
+      ECHK(B.res_block(b.res, cur, nullptr, 1e-5f, r));
+      ECHK(transformer(b, r));
       cur = r;
-    } else {
-      const int Ho = (cur.h + 2 - 3) / 2 + 1, Wo = (cur.w + 2 - 3) / 2 + 1;
-      Act d = B.new_act(n, Ho, Wo, b.ch_out);
-      ECHK(B.conv3(cur, b.down, d.p, b.ch_out, Builder::GemmOpt(), 2, 1, Ho, Wo));
-      cur = d;
+      hs.push_back(cur);
     }
-    hs.push_back(cur);
+    if (lv.has_down) {
+      const int Ho = (cur.h + 2 - 3) / 2 + 1, Wo = (cur.w + 2 - 3) / 2 + 1;
+      Act d = B.new_act(n, Ho, Wo, lv.down.N);
+      ECHK(B.conv3(cur, lv.down, d.p, lv.down.N, Builder::GemmOpt(), 2, 1, Ho, Wo));
+      cur = d;
+      hs.push_back(cur);
+    }
   }
-  // ---- middle
-  {
-    Act r1, t, r2;
-    ECHK(B.res_block(e->mid_r1, cur, nullptr, emb_ptr, ld_emb, 1e-5f, r1));
-    ECHK(B.spatial_transformer(e->mid_st, r1, kvbuf.p, e->kv_total, ctx_len, t));
-    B.free_act(r1);
-    ECHK(B.res_block(e->mid_r2, t, nullptr, emb_ptr, ld_emb, 1e-5f, r2));
-    B.free_act(t);
-    cur = r2;  // note: hs.back() (same tensor as the old cur) is still owned by the skip stack
-  }
+  // ---- middle (its input, the last input block's output, stays on the skip stack)
+  Act r;
+  ECHK(B.res_block(u.mid_r1, cur, nullptr, 1e-5f, r));
+  ECHK(B.spatial_transformer(u.mid_st, r, kvbuf.p, u.kv_total, ctx_len));
+  ECHK(B.res_replace(u.mid_r2, r, 1e-5f));
+  cur = r;
   // ---- output blocks
-  bool cur_owned = true;
-  for (size_t bi = 0; bi < e->out_blocks.size(); ++bi) {
-    const BlockW& b = e->out_blocks[bi];
+  for (const UNetBlockW& b : u.out_blocks) {
     Act skip = hs.back();
     hs.pop_back();
     if (skip.h != cur.h || skip.w != cur.w) EFAIL("unet: skip / hidden size mismatch (latent size must be divisible by 2^(levels-1))");
-    Act r;
-    ECHK(B.res_block(b.res, cur, &skip, emb_ptr, ld_emb, 1e-5f, r));
-    if (cur_owned) B.free_act(cur);
+    ECHK(B.res_replace(b.res, cur, 1e-5f, &skip));
     B.free_act(skip);
-    if (b.has_st) {
-      Act t;
-      ECHK(B.spatial_transformer(b.st, r, kvbuf.p, e->kv_total, ctx_len, t));
-      B.free_act(r);
-      r = t;
-    }
-    if (b.has_up) {
-      Act c;
-      ECHK(B.upsample_conv(r, b.up, c));
-      r = c;
-    }
-    cur = r;
-    cur_owned = true;
+    ECHK(transformer(b, cur));
+    if (b.has_up) ECHK(B.upsample_conv(cur, b.up));
   }
   // ---- out: GN + SiLU + conv3 -> [M, 8] (4 valid channels)
-  ECHK(B.out_head(cur, e->out_norm, 1e-5f, e->out_conv));
+  ECHK(B.out_head(cur, u.out_norm, 1e-5f, u.out_conv));
   // plan-owned buffers (conv_in's im2col, ctx16, temb, y32, e1, emb, l1, emb_all, kvbuf, out_head's output) stay reserved for this plan
   return 0;
 }
@@ -1266,71 +1276,37 @@ __global__ void post_quant_kernel(const void* __restrict__ z, int io_dtype, cons
   }
 }
 
-// AttnBlock (sd_hijack_optimizations.py:637-655): GN -> fused q|k|v 1x1 conv -> single-head attention -> proj + x
-int vae_attn_block(sdxe_engine* e, Builder& B, Act& cur, const NormW& norm, const LinW& qkv_w, const LinW& proj_w) {
-  const int C = cur.c, tokens = cur.h * cur.w, n = cur.n;
-  const int64_t M = cur.rows();
-  Act xn;
-  ECHK(B.group_norm(cur, nullptr, norm, 1e-6f, false, xn));
-  Buf qkv = e->alloc((size_t)M * 3 * C * 2);
-  ECHK(B.gemm(xn.p, C, M, qkv_w, qkv.p, Builder::GemmOpt()));
-  B.free_act(xn);
-  if (C % 64 != 0 || C > 512) EFAIL("vae attention: channel count must be a multiple of 64 and <= 512");
-  Act att = B.new_act(n, cur.h, cur.w, C);
-  const uint16_t* qp = (const uint16_t*)qkv.p;
-  ECHK(B.attention(qp, qp + C, qp + 2 * C, n, 1, tokens, tokens, C, 3 * C, 3 * C, 1.0f / sqrtf((float)C), att.p, C, C));
-  e->release(qkv);
-  Act o = B.new_act(n, cur.h, cur.w, C);
-  Builder::GemmOpt op;
-  op.residual = cur.p; op.ldr = C;
-  ECHK(B.gemm(att.p, C, M, proj_w, o.p, op));
-  B.free_act(att);
-  B.free_act(cur);
-  cur = o;
-  return 0;
-}
-
 // AutoencoderKL.encode up to the moments: x [n, 3, H, W] -> [n, 2z, H/8, W/8]
 int build_vae_encode_plan(sdxe_engine* e, Plan* p, int n, int H, int W) {
   const sdxe_config& cfg = e->cfg;
+  const VaeW& v = *e->vae;
   Builder B(e, p);
   const bool bf16 = e->bf16;
-  const int nl = cfg.num_levels, cin = cfg.vae_out_ch, z2 = 2 * cfg.vae_z_channels;
+  const int z2 = 2 * cfg.vae_z_channels;
   Act cur;
-  ECHK(B.conv_in_nchw(nullptr, n, cin, H, W, e->e_conv_in, cur));
-  Act t;
-  for (int level = 0; level < nl; ++level) {
-    for (const ResW& r : e->e_down_blocks[level]) {
-      ECHK(B.res_block(r, cur, nullptr, nullptr, 0, 1e-6f, t));
-      B.free_act(cur);
-      cur = t;
-    }
-    if (level != nl - 1) {
+  ECHK(B.conv_in_nchw(nullptr, n, cfg.vae_out_ch, H, W, v.conv_in, cur));
+  for (const VaeLevelW& lv : v.levels) {
+    for (const ResW& r : lv.blocks) ECHK(B.res_replace(r, cur, 1e-6f));
+    if (lv.has_resample) {
       // ldm Downsample (with_conv): pad (0,1,0,1) then conv3x3 stride 2, padding 0 -> taps start at the pixel itself
       const int Ho = cur.h / 2, Wo = cur.w / 2;
       Act d = B.new_act(n, Ho, Wo, cur.c);
-      ECHK(B.conv3(cur, e->e_down_conv[level], d.p, cur.c, Builder::GemmOpt(), 2, 0, Ho, Wo));
+      ECHK(B.conv3(cur, lv.resample, d.p, cur.c, Builder::GemmOpt(), 2, 0, Ho, Wo));
       B.free_act(cur);
       cur = d;
     }
   }
-  ECHK(B.res_block(e->e_mid1, cur, nullptr, nullptr, 0, 1e-6f, t));
-  B.free_act(cur);
-  cur = t;
-  ECHK(vae_attn_block(e, B, cur, e->e_attn_norm, e->e_qkv, e->e_proj));
-  ECHK(B.res_block(e->e_mid2, cur, nullptr, nullptr, 0, 1e-6f, t));
-  B.free_act(cur);
-  cur = t;
+  ECHK(B.vae_mid(v.mid, cur));
   Act g;
-  ECHK(B.group_norm(cur, nullptr, e->e_norm_out, 1e-6f, true, g));
+  ECHK(B.group_norm(cur, nullptr, v.norm_out, 1e-6f, true, g));
   const int Ho = cur.h, Wo = cur.w;
   B.free_act(cur);
   const int ld8 = (int)align_up(z2, 8);
   Act mo = B.new_act(n, Ho, Wo, ld8);
-  ECHK(B.conv3(g, e->e_conv_out, mo.p, ld8, Builder::GemmOpt()));
+  ECHK(B.conv3(g, v.conv_out, mo.p, ld8, Builder::GemmOpt()));
   B.free_act(g);
   Buf outb = e->alloc((size_t)n * Ho * Wo * ld8 * 2);
-  ECHK(B.gemm(mo.p, ld8, (int64_t)n * Ho * Wo, e->e_quant, outb.p, Builder::GemmOpt()));  // quant_conv (1x1)
+  ECHK(B.gemm(mo.p, ld8, (int64_t)n * Ho * Wo, v.quant, outb.p, Builder::GemmOpt()));  // quant_conv (1x1)
   B.free_act(mo);
   {
     void* ob = outb.p;
@@ -1341,14 +1317,14 @@ int build_vae_encode_plan(sdxe_engine* e, Plan* p, int n, int H, int W) {
 }
 
 int build_vae_plan(sdxe_engine* e, Plan* p, int n, int h, int w) {
-  const sdxe_config& cfg = e->cfg;
+  const VaeW& v = *e->vae;
   Builder B(e, p);
   const bool bf16 = e->bf16;
-  const int z = cfg.vae_z_channels, nl = cfg.num_levels;
+  const int z = e->cfg.vae_z_channels;
   Buf zq = e->alloc((size_t)n * h * w * z * 2);
   {
     void* zp = zq.p;
-    const float *pw = e->pq_w, *pb = e->pq_b;
+    const float *pw = v.pq_w, *pb = v.pq_b;
     const int hw = h * w;
     p->pre.push_back([=](cudaStream_t s) {
       const int64_t total = (int64_t)n * z * hw;
@@ -1360,39 +1336,19 @@ int build_vae_plan(sdxe_engine* e, Plan* p, int n, int h, int w) {
     });
   }
   Act cur;
-  ECHK(B.conv_in_nchw(zq.p, n, z, h, w, e->v_conv_in, cur));
-  Act t;
-  ECHK(B.res_block(e->v_mid1, cur, nullptr, nullptr, 0, 1e-6f, t));
-  B.free_act(cur);
-  cur = t;
-  ECHK(vae_attn_block(e, B, cur, e->v_attn_norm, e->v_qkv, e->v_proj));
-  ECHK(B.res_block(e->v_mid2, cur, nullptr, nullptr, 0, 1e-6f, t));
-  B.free_act(cur);
-  cur = t;
-  for (int level = nl - 1; level >= 0; --level) {
-    for (const ResW& r : e->v_up_blocks[level]) {
-      ECHK(B.res_block(r, cur, nullptr, nullptr, 0, 1e-6f, t));
-      B.free_act(cur);
-      cur = t;
-    }
-    if (level != 0) {
-      ECHK(B.upsample_conv(cur, e->v_up_conv[level], t));
-      cur = t;
-    }
+  ECHK(B.conv_in_nchw(zq.p, n, z, h, w, v.conv_in, cur));
+  ECHK(B.vae_mid(v.mid, cur));
+  for (auto lv = v.levels.rbegin(); lv != v.levels.rend(); ++lv) {
+    for (const ResW& r : lv->blocks) ECHK(B.res_replace(r, cur, 1e-6f));
+    if (lv->has_resample) ECHK(B.upsample_conv(cur, lv->resample));
   }
-  return B.out_head(cur, e->v_norm_out, 1e-6f, e->v_conv_out);
+  return B.out_head(cur, v.norm_out, 1e-6f, v.conv_out);
 }
-
-}  // namespace
-
-// =================================================================================================================
-// C-ABI
-// =================================================================================================================
-namespace {
 
 // hidden_states[layer] (optionally + final_layer_norm) of the text transformer for n sequences of T tokens
 int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int final_norm) {
   const sdxe_config& cfg = e->cfg;
+  const ClipW& c = *e->clip;
   const int C = cfg.clip_hidden, I = cfg.clip_intermediate, H = cfg.clip_heads, d = C / H;
   const int64_t M = (int64_t)n * T;
   const bool b = e->bf16;
@@ -1405,7 +1361,7 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
   {
     void* xp = x.p;
     float2* sp = (float2*)st.buf.p;
-    const void *tok = e->c_tok, *pos = e->c_pos;
+    const void *tok = c.tok, *pos = c.pos;
     const int vocab = cfg.clip_vocab;
     plan->pre.push_back([=](cudaStream_t s) {
       ECHK(clip_embed_launch((const int32_t*)plan->x, tok, pos, xp, sp, (int)M, T, C, vocab, b, s));
@@ -1414,7 +1370,7 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
   }
   const float scale = 1.0f / sqrtf((float)d);
   for (int l = 0; l < layer; ++l) {
-    const ClipLayerW& w = e->c_layers[l];
+    const ClipLayerW& w = c.layers[l];
     Buf qkv = e->alloc((size_t)M * 3 * C * 2);
     Builder::GemmOpt oq;
     oq.ln_part = st.p; oq.ln_parts = st.parts;
@@ -1461,7 +1417,7 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
     y = e->alloc((size_t)M * C * 2);
     const void* xp = x.p;
     void* yp = y.p;
-    const float *g = e->c_final.g, *bt = e->c_final.b;
+    const float *g = c.final_norm.g, *bt = c.final_norm.b;
     B.ops->push_back(OpRec([=](cudaStream_t s) { return layer_norm_launch(xp, g, bt, yp, (int)M, C, 1e-5f, b, s); }, K_LNORM, 0.0,
                            4.0 * (double)M * C, "final_layer_norm"));
   }
@@ -1477,10 +1433,9 @@ int build_clip_plan(sdxe_engine* e, Plan* plan, int n, int T, int layer, int fin
   return 0;
 }
 
-}  // namespace
-
-namespace {
-
+// =================================================================================================================
+// plan cache
+// =================================================================================================================
 // Drop the least recently used plan: its graph is destroyed and the buffers it pinned go back to the pool; pool memory
 // beyond pool_limit is returned to the driver (largest blocks first).
 void evict_lru(sdxe_engine* e) {
@@ -1552,8 +1507,36 @@ Plan* get_plan(sdxe_engine* e, const std::string& key, BuildFn build) {
   return nullptr;
 }
 
+// One model forward: `e` must be a finalized engine of `kind` and io_dtype a type it reads and writes; `args` checks the
+// remaining arguments and may extend the plan key; the plan for the key is fetched or built, gets this call's pointers
+// (x, out, io_dtype, then `bind`) and runs on `stream`. `entry` / `model` name the call and the model in error messages.
+int run_forward(sdxe_engine* e, int kind, const char* entry, const char* model, int io_dtype, std::string key,
+                const std::function<int(std::string& key)>& args, const std::function<int(Plan*)>& build, const void* x,
+                void* out, void* stream, const std::function<void(Plan*)>& bind = nullptr) {
+  if (!e || !e->finalized || e->cfg.kind != kind) EFAIL((std::string(entry) + ": engine is not a finalized " + model).c_str());
+  if (kind == SDXE_MODEL_CLIP_TEXT ? io_dtype != e->dt && io_dtype != SDXE_F32
+                                   : io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32)
+    EFAIL((std::string(entry) + (kind == SDXE_MODEL_CLIP_TEXT ? ": out must be the engine's 16-bit type or fp32" : ": io dtype")).c_str());
+  ECHK(args(key));
+  if (e->circular) key += ":circ";  // only UNet and VAE engines take Tiling (sdxe_set_circular)
+  Plan* p = get_plan(e, key, build);
+  if (!p) return -1;
+  p->x = x; p->out = out; p->io_dtype = io_dtype;
+  if (bind) bind(p);
+  return run_plan(e, p, (cudaStream_t)stream);
+}
+
+std::string dims_key(char tag, std::initializer_list<int> dims) {
+  std::string key(1, tag);
+  for (int d : dims) key += ":" + std::to_string(d);
+  return key;
+}
+
 }  // namespace
 
+// =================================================================================================================
+// C-ABI
+// =================================================================================================================
 extern "C" {
 
 int sdxe_create(const sdxe_config* cfg, sdxe_engine** out) {
@@ -1578,6 +1561,11 @@ int sdxe_create(const sdxe_config* cfg, sdxe_engine** out) {
   e->cfg = *cfg;
   e->bf16 = cfg->dtype == SDXE_BF16;
   e->dt = cfg->dtype;
+  switch (cfg->kind) {
+    case SDXE_MODEL_UNET: e->unet.reset(new UNetW()); break;
+    case SDXE_MODEL_CLIP_TEXT: e->clip.reset(new ClipW()); break;
+    default: e->vae.reset(new VaeW()); break;
+  }
   if (gemm_init() != 0 || attention_init() != 0 || kernels_init() != 0) { delete e; return -1; }
   *out = e;
   return 0;
@@ -1619,8 +1607,13 @@ int sdxe_finalize(sdxe_engine* e) {
     e->sizing = pass == 0;
     e->cursor = 0;
     e->missing.clear();
-    int rc = e->cfg.kind == SDXE_MODEL_UNET ? e->build_unet()
-             : (e->cfg.kind == SDXE_MODEL_VAE_ENCODER ? e->build_vae_encoder() : (e->cfg.kind == SDXE_MODEL_CLIP_TEXT ? e->build_clip() : e->build_vae()));
+    int rc;
+    switch (e->cfg.kind) {
+      case SDXE_MODEL_UNET: rc = e->build_unet(*e->unet); break;
+      case SDXE_MODEL_VAE_ENCODER: rc = e->build_vae_encoder(*e->vae); break;
+      case SDXE_MODEL_CLIP_TEXT: rc = e->build_clip(*e->clip); break;
+      default: rc = e->build_vae_decoder(*e->vae); break;
+    }
     if (rc != 0) return -1;
     if (!e->missing.empty()) {
       std::string m = "sdxe_finalize: missing / mis-shaped weights: " + e->missing;
@@ -1651,21 +1644,15 @@ int sdxe_weight_blob(sdxe_engine* e, void** device_ptr, int64_t* bytes) {
 
 int sdxe_unet_forward(sdxe_engine* e, const void* x, const void* t, const void* ctx, const void* y, void* out, int n,
                       int h, int w, int ctx_len, int io_dtype, void* stream) {
-  if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_forward: engine is not a finalized UNet");
-  if (!x || !t || !ctx || !out || n <= 0 || h <= 0 || w <= 0 || ctx_len <= 0) EFAIL("sdxe_unet_forward: bad argument");
-  if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_unet_forward: io dtype");
-  std::string key = "u:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + ":" + std::to_string(ctx_len);
   std::vector<int32_t> ht;
-  ht.swap(e->ht_rows);  // a Hypertile table applies to one call
   HtDraws draws;
-  if (!ht.empty()) {
+  auto args = [&](std::string& key) {
+    if (!x || !t || !ctx || !out || n <= 0 || h <= 0 || w <= 0 || ctx_len <= 0) EFAIL("sdxe_unet_forward: bad argument");
+    ht.swap(e->unet->ht_rows);  // a Hypertile table applies to one call
+    if (ht.empty()) return 0;
     // the plan is keyed on the structural part (h', w', max_tiles per layer); the draws (nh, nw) are data
-    int n_attn1 = (int)e->mid_st.blocks.size();
-    for (const auto* blocks : {&e->in_blocks, &e->out_blocks})
-      for (const BlockW& b : *blocks)
-        if (b.has_st) n_attn1 += (int)b.st.blocks.size();
     draws.n = (int)ht.size() / 5;
-    if (draws.n != n_attn1) EFAIL("sdxe_unet_forward: the Hypertile table needs one row per attn1 layer");
+    if (draws.n != e->unet->n_attn1) EFAIL("sdxe_unet_forward: the Hypertile table needs one row per attn1 layer");
     key += ":ht";
     for (int i = 0; i < draws.n; ++i) {
       const int32_t* r = &ht[5 * i];
@@ -1676,13 +1663,14 @@ int sdxe_unet_forward(sdxe_engine* e, const void* x, const void* t, const void* 
       draws.v[2 * i + 1] = nw;
       key += mt > 0 ? "," + std::to_string(hp) + "x" + std::to_string(wp) + "/" + std::to_string(mt) : ",-";
     }
-  }
-  if (e->circular) key += ":circ";
-  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_unet_plan(e, pl, n, h, w, ctx_len, ht.empty() ? nullptr : &ht); });
-  if (!p) return -1;
-  if (!ht.empty()) p->ht_draws = draws;
-  p->x = x; p->t = t; p->ctx = ctx; p->y = y; p->out = out; p->io_dtype = io_dtype;
-  return run_plan(e, p, (cudaStream_t)stream);
+    return 0;
+  };
+  return run_forward(e, SDXE_MODEL_UNET, "sdxe_unet_forward", "UNet", io_dtype, dims_key('u', {n, h, w, ctx_len}), args,
+                     [&](Plan* pl) { return build_unet_plan(e, pl, n, h, w, ctx_len, ht.empty() ? nullptr : &ht); }, x, out, stream,
+                     [&](Plan* p) {
+                       if (!ht.empty()) p->ht_draws = draws;
+                       p->t = t; p->ctx = ctx; p->y = y;
+                     });
 }
 
 int sdxe_clip_forward(sdxe_engine* e, const int32_t* tokens, void* out, int n, int T, int layer, int final_norm, int io_dtype,
@@ -1692,28 +1680,27 @@ int sdxe_clip_forward(sdxe_engine* e, const int32_t* tokens, void* out, int n, i
 
 int sdxe_clip_forward_fixes(sdxe_engine* e, const int32_t* tokens, void* out, int n, int T, int layer, int final_norm, int io_dtype,
                             const int32_t* fix_rows, const void* fix_vecs, int n_fix, void* stream) {
-  if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_CLIP_TEXT) EFAIL("sdxe_clip_forward: engine is not a finalized CLIP text model");
-  if (!tokens || !out || n <= 0 || T <= 0 || T > e->cfg.clip_positions || layer < 0 || layer > e->cfg.clip_layers) EFAIL("sdxe_clip_forward: bad argument");
-  if (io_dtype != e->dt && io_dtype != SDXE_F32) EFAIL("sdxe_clip_forward: out must be the engine's 16-bit type or fp32");
-  const std::string key = "c:" + std::to_string(n) + ":" + std::to_string(T) + ":" + std::to_string(layer) + ":" + std::to_string(final_norm ? 1 : 0);
-  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_clip_plan(e, pl, n, T, layer, final_norm ? 1 : 0); });
-  if (!p) return -1;
-  if (n_fix < 0 || (n_fix > 0 && (!fix_rows || !fix_vecs))) EFAIL("sdxe_clip_forward_fixes: bad fix arguments");
-  p->x = tokens; p->out = out; p->io_dtype = io_dtype;
-  p->fix_rows = fix_rows; p->fix_vecs = fix_vecs; p->n_fix = n_fix;
-  return run_plan(e, p, (cudaStream_t)stream);
+  const int fnorm = final_norm ? 1 : 0;
+  auto args = [&](std::string&) {
+    if (!tokens || !out || n <= 0 || T <= 0 || T > e->cfg.clip_positions || layer < 0 || layer > e->cfg.clip_layers) EFAIL("sdxe_clip_forward: bad argument");
+    if (n_fix < 0 || (n_fix > 0 && (!fix_rows || !fix_vecs))) EFAIL("sdxe_clip_forward_fixes: bad fix arguments");
+    return 0;
+  };
+  return run_forward(e, SDXE_MODEL_CLIP_TEXT, "sdxe_clip_forward", "CLIP text model", io_dtype, dims_key('c', {n, T, layer, fnorm}),
+                     args, [&](Plan* pl) { return build_clip_plan(e, pl, n, T, layer, fnorm); }, tokens, out, stream,
+                     [&](Plan* p) { p->fix_rows = fix_rows; p->fix_vecs = fix_vecs; p->n_fix = n_fix; });
 }
 
 int sdxe_unet_set_context_key(sdxe_engine* e, int64_t key) {
   if (!e || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_set_context_key: not a UNet engine");
-  e->ctx_key = key;
+  e->unet->ctx_key = key;
   return 0;
 }
 
 int sdxe_unet_set_hypertile(sdxe_engine* e, const int32_t* layers, int n_layers) {
   if (!e || e->cfg.kind != SDXE_MODEL_UNET) EFAIL("sdxe_unet_set_hypertile: not a UNet engine");
   if (n_layers < 0 || n_layers > HT_MAX_LAYERS || (n_layers > 0 && !layers)) EFAIL("sdxe_unet_set_hypertile: bad argument");
-  e->ht_rows.assign(layers, layers + 5 * n_layers);
+  e->unet->ht_rows.assign(layers, layers + 5 * n_layers);
   return 0;
 }
 
@@ -1758,26 +1745,22 @@ int sdxe_profile_read(sdxe_engine* e, int kind, double* ms, double* flops, doubl
 }
 
 int sdxe_vae_decode(sdxe_engine* e, const void* z, void* out, int n, int h, int w, int io_dtype, void* stream) {
-  if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_VAE_DECODER) EFAIL("sdxe_vae_decode: engine is not a finalized VAE decoder");
-  if (!z || !out || n <= 0 || h <= 0 || w <= 0) EFAIL("sdxe_vae_decode: bad argument");
-  if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_vae_decode: io dtype");
-  const std::string key = "v:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + (e->circular ? ":circ" : "");
-  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_vae_plan(e, pl, n, h, w); });
-  if (!p) return -1;
-  p->x = z; p->out = out; p->io_dtype = io_dtype;
-  return run_plan(e, p, (cudaStream_t)stream);
+  auto args = [&](std::string&) {
+    if (!z || !out || n <= 0 || h <= 0 || w <= 0) EFAIL("sdxe_vae_decode: bad argument");
+    return 0;
+  };
+  return run_forward(e, SDXE_MODEL_VAE_DECODER, "sdxe_vae_decode", "VAE decoder", io_dtype, dims_key('v', {n, h, w}), args,
+                     [&](Plan* pl) { return build_vae_plan(e, pl, n, h, w); }, z, out, stream);
 }
 
 int sdxe_vae_encode(sdxe_engine* e, const void* x, void* out, int n, int h, int w, int io_dtype, void* stream) {
-  if (!e || !e->finalized || e->cfg.kind != SDXE_MODEL_VAE_ENCODER) EFAIL("sdxe_vae_encode: engine is not a finalized VAE encoder");
-  const int f = 1 << (e->cfg.num_levels - 1);  // spatial reduction of the encoder (8 for the SD VAE)
-  if (!x || !out || n <= 0 || h <= 0 || w <= 0 || (h % f) || (w % f)) EFAIL("sdxe_vae_encode: bad argument (H, W must be multiples of the encoder's downsampling factor)");
-  if (io_dtype != SDXE_F16 && io_dtype != SDXE_BF16 && io_dtype != SDXE_F32) EFAIL("sdxe_vae_encode: io dtype");
-  const std::string key = "e:" + std::to_string(n) + ":" + std::to_string(h) + ":" + std::to_string(w) + (e->circular ? ":circ" : "");
-  Plan* p = get_plan(e, key, [&](Plan* pl) { return build_vae_encode_plan(e, pl, n, h, w); });
-  if (!p) return -1;
-  p->x = x; p->out = out; p->io_dtype = io_dtype;
-  return run_plan(e, p, (cudaStream_t)stream);
+  auto args = [&](std::string&) {
+    const int f = 1 << (e->cfg.num_levels - 1);  // spatial reduction of the encoder (8 for the SD VAE)
+    if (!x || !out || n <= 0 || h <= 0 || w <= 0 || (h % f) || (w % f)) EFAIL("sdxe_vae_encode: bad argument (H, W must be multiples of the encoder's downsampling factor)");
+    return 0;
+  };
+  return run_forward(e, SDXE_MODEL_VAE_ENCODER, "sdxe_vae_encode", "VAE encoder", io_dtype, dims_key('e', {n, h, w}), args,
+                     [&](Plan* pl) { return build_vae_encode_plan(e, pl, n, h, w); }, x, out, stream);
 }
 
 }  // extern "C"
